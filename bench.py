@@ -15,6 +15,9 @@ from pinned HOST buffers (H2D of X and the class labels inside the timed region;
 async copies while the fit runs) -- DESIGN.md section 7.
 `--impl reference` times the CPU stand-in for the reference (the numpy/OpenBLAS fp64 oracle: the reference's own
 Spark/Breeze path needs a JVM that this image does not have) on a bounded row sample of the same workload.
+`--dump-outputs DIR` writes the model the last timed step of each resident leg returned (the inputs are seeded, so two builds
+run with the same arguments can be compared array by array): `{mode}_W_sample.npy` (a fixed, seeded sample of 2048 rows of
+the D x k weights), `{mode}_feature_means.npy` (D) and `{mode}_intercept.npy` (k), all float64.
 """
 from __future__ import annotations
 
@@ -66,7 +69,21 @@ def parse_args():
     ap.add_argument("--no-fast-mode", action="store_true")
     ap.add_argument("--precision", default=os.environ.get("KS_BENCH_PRECISION", "f16x2"), choices=["tf32", "f16", "f16x2"],
                     help="operand mode of the top-level numbers (fp32 accumulate, fp64 solve in every mode)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the model of the last timed step of each resident leg to DIR/<name>.npy")
     return ap.parse_args()
+
+
+DUMP_W_ROWS = 2048   # rows of W kept by --dump-outputs (2 modes x 2048 x k=1000 x 8 B = 33 MB at the default shape)
+
+
+def model_outputs(model, mode):
+    """The arrays a caller of fit() receives, copied out of the pinned mirror (the next fit reuses it); W is sampled."""
+    W = np.concatenate(model.xs, 0)
+    rows = np.sort(np.random.default_rng(0).choice(W.shape[0], min(DUMP_W_ROWS, W.shape[0]), replace=False))
+    return {f"{mode}_W_sample": W[rows].astype(np.float64),
+            f"{mode}_feature_means": np.concatenate(model.feature_means).astype(np.float64),
+            f"{mode}_intercept": np.asarray(model.b_opt, dtype=np.float64).copy()}
 
 
 # ----------------------------------------------------------------------------------------- workload
@@ -296,17 +313,22 @@ def main():
             sampler.start()
         l0 = ctx.launch_count()
         stats, step_wall = [], []
+        model = None
         t0 = time.perf_counter()
         for _ in range(steps):
             ts = time.perf_counter()
-            touch(est.fit(feats, y_dev))
+            model = est.fit(feats, y_dev)
+            touch(model)
             step_wall.append(1e3 * (time.perf_counter() - ts))
             stats.append(ctx.last_fit_stats())
         barrier()
         t = max_over_ranks((time.perf_counter() - t0) / steps)
+        if args.dump_outputs and rank == 0:
+            dumps.update(model_outputs(model, precision))
         return {"t": t, "launches": (ctx.launch_count() - l0) // max(steps, 1), "clocks": sampler.stop() if sampler else None,
                 "dev_ms": max_over_ranks(float(np.mean([s["total_ms"] for s in stats]))), "step_wall": step_wall, "stats": stats[-1]}
 
+    dumps = {}
     main_leg = resident_leg(args.precision, args.steps, args.warmup, True)
     fast_leg = None
     if args.precision != "f16" and not args.no_fast_mode:
@@ -394,37 +416,24 @@ def main():
             dist.destroy_process_group()
         return
 
-    # ---- roofline of the dominant kernel (gram2_tn_kernel), timed alone with CUDA events (above)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except OSError:
-        pass
-    peak = peaks.get("bf16_tflops") or 1700.0
-    peak_src = ("MEASURED_PEAKS.json bf16_tflops (burst: the kernel is timed alone)" if peaks else
-                "fallback 1.7 PFLOP/s dense bf16 burst (B200_PROFILING.md)")
+    # ---- roofline of the dominant kernel (gram_tn_kernel), timed alone with CUDA events (above)
+    tf32 = args.precision == "tf32"
+    peak = 494.7 if tf32 else 989.4   # NVIDIA H100 SXM data sheet, dense, 700 W board power: a ceiling, not a measured rate
+    peak_src = f"H100 SXM data sheet, dense {'tf32' if tf32 else 'fp16'} at 700 W (a card set to a lower power limit clocks lower)"
     n_loc = hi - lo
     gram_launch_flops = 2.0 * n_loc * args.block * (args.block + args.classes)          # full-GEMM convention, per launch
     achieved = gram_launch_flops / (gram_ms * 1e-3) / 1e12
-    executed = None
-    if args.block == 4096 and args.classes == 1000:
-        executed = achieved * (104 * 256 * 512) / (args.block * (args.block + args.classes))   # 72 G + 32 C pair tiles of 256 x 512
-    traffic, traffic_ref = None, None
-    try:
-        traffic_ref = json.load(open(os.path.join(ROOT, "profiles", "gram_ncu_summary.json")))
-        if traffic_ref.get("n_rows") == n_loc:
-            traffic = traffic_ref.get("dram_bytes_per_launch")
-    except (OSError, ValueError):
-        pass
-    kind = "kind::tf32" if args.precision == "tf32" else "kind::f16"
-    roofline = {"kernel": f"gram2_tn_kernel (tcgen05 cta_group::2 {kind}, S^T [S | R])", "bound": "tensor", "achieved": achieved,
-                "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
-                "executed_tflops": executed, "executed_frac": executed / peak if executed else None,
+    mb = -(-args.block // 128)
+    tiles = mb * (mb + 1) // 2 + mb * -(-args.classes // 128)   # 128 x 128 tiles: upper triangle of G, all of C
+    executed = achieved * (tiles * 128 * 128) / (args.block * (args.block + args.classes))
+    kind = "tf32 mma.sync" if tf32 else "fp16 wgmma"
+    roofline = {"kernel": f"gram_tn_kernel ({kind}, S^T [S | R])", "bound": "tensor", "achieved": achieved,
+                "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "peak_source": peak_src,
+                "executed_tflops": executed, "executed_frac": executed / peak,
                 "note": "achieved = ALGORITHMIC flops 2*N_loc*b*(b+k) per launch (full-GEMM convention of the reference cost model, "
-                        "SURVEY 8d) / mean launch duration; the kernel skips the lower triangle of G, so executed MMA flops are "
-                        "0.65x of that: executed_tflops / executed_frac are the figures to hold against the tensor peak (the tf32 "
-                        "MMA rate is half the bf16 / fp16 rate)",
-                "ms_per_launch": gram_ms, "traffic_reference_capture": traffic_ref}
+                        "SURVEY 8d) / mean launch duration; the kernel skips the lower triangle of G, so it executes fewer MMA "
+                        "flops than that: executed_tflops / executed_frac are the figures to hold against the tensor peak",
+                "ms_per_launch": gram_ms}
 
     cpu_baseline = None
     if world == 1 and not args.no_cpu_baseline:
@@ -456,6 +465,11 @@ def main():
         out["parity"] = parity
     if cpu_baseline:
         out["cpu_baseline"] = cpu_baseline
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dumps.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
+        out["dumped_outputs"] = sorted(dumps)
     print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()

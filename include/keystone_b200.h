@@ -1,4 +1,4 @@
-/* keystone_b200 -- C ABI of the B200-native block least-squares engine.
+/* keystone_b200 -- C ABI of the H100-native (sm_90a) block least-squares engine.
  *
  * Drop-in boundary for the KeystoneML (amplab/keystone) node bodies on the block-LS hot path.
  * Every entry point names the reference interface it replaces (paths relative to
@@ -55,12 +55,12 @@ extern "C" {
 #define KS_PRECISION_DEFAULT (-1) /* the context's setting (ks_ctx_set_option "precision"; initial value KS_PRECISION_F16X2) */
 #define KS_PRECISION_TF32 0  /* one tf32 MMA per product: operands rounded to tf32 (10-bit mantissa, round-to-nearest) */
 #define KS_PRECISION_F16 1   /* fast mode.  Generated (cosine) features: fp16 operands (same 10-bit mantissa as tf32, residual /
-                                increments scaled by device-chosen powers of two), kind::f16 MMA at twice the tf32 rate;
+                                increments scaled by device-chosen powers of two), fp16 wgmma at twice the tf32 rate;
                                 materialised feature matrices fall back to KS_PRECISION_TF32 */
 #define KS_PRECISION_F16X2 2 /* parity mode (split operands): every MMA operand v is carried as hi + lo (hi = round(v),
                                 lo = round(v - hi): >= 21 significant bits) and every product keeps hi*hi + hi*lo + lo*hi on the
-                                same kernels.  Generated features: fp16 pairs (kind::f16, ~3x the fast mode's tensor work);
-                                materialised feature matrices: tf32 pairs (kind::tf32).  Measured against the fp64 oracle:
+                                same kernels.  Generated features: fp16 pairs (fp16 MMA, ~3x the fast mode's tensor work);
+                                materialised feature matrices: tf32 pairs (tf32 MMA).  Measured against the fp64 oracle:
                                 see DESIGN.md section 6 */
 
 #define KS_NCCL_ID_BYTES 128
@@ -78,8 +78,7 @@ KS_API const char* ks_last_error(int64_t ctx);
 KS_API int32_t ks_ctx_synchronize(int64_t ctx);
 /* tunables (defaults in brackets): "gram_chunk_rows" [0 = chosen from the local row count], "sample_rows" [16384: rows per rank
  * for the shift estimate of generated features], "precision" [2 = KS_PRECISION_F16X2: what KS_PRECISION_DEFAULT and the entry
- * points without a precision argument use], "gram_pair" [1: cta_group::2 kernels], "epi_multi" [1: rotating epilogue staging
- * buffers], "proj_f16" [1: fp16 projection operands in fp16 mode], "shard_solve" [1: triangular solves sharded by
+ * points without a precision argument use], "proj_f16" [1: fp16 projection operands in fp16 mode], "shard_solve" [1: triangular solves sharded by
  * right-hand-side columns over the ranks], "reserve_sms" [8], "timing" [1], "pipeline" [1: all tensor-core kernels of a fit on
  * one stream, solve / factor chains beside it; 0: the two-stream arrangement of round 1], "host_mirror" [1: fits copy each
  * finished model block into pinned host memory while they run]; "custom_solve" [-1: automatic -- the library's own DMMA

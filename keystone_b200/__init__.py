@@ -1,7 +1,7 @@
-"""keystone_b200 -- B200-native block least-squares engine behind the KeystoneML node API.
+"""keystone_b200 -- H100-native block least-squares engine behind the KeystoneML node API.
 
 The package is a thin host layer over ``lib/libkeystone_b200.so`` (C ABI in ``include/keystone_b200.h``);
-all numerics run in hand-written sm_100a kernels.  There is no CPU fallback.
+all numerics run in hand-written sm_90a kernels.  There is no CPU fallback.
 """
 from ._capi import KeystoneError, LIB_PATH, declared_symbols  # noqa: F401
 from .context import Context, DeviceMatrix, LazyFeatures, shard_range  # noqa: F401

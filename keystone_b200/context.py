@@ -1,6 +1,6 @@
 """GPU context and row-sharded device datasets (host side of the C ABI).
 
-``Context`` = one process / one B200 (``ks_ctx_create``).  ``DeviceMatrix`` is this rank's shard of
+``Context`` = one process / one GPU (``ks_ctx_create``).  ``DeviceMatrix`` is this rank's shard of
 a row-partitioned dataset -- the stand-in for the reference's ``RDD[DenseVector[Double]]`` at the
 estimator boundary (SURVEY.md 8a/a11).  ``LazyFeatures`` is the un-materialised output of gathered
 CosineRandomFeatures nodes: the fit regenerates every feature block from ``x_in`` instead of storing

@@ -15,7 +15,7 @@ __device__ __forceinline__ float round_tf32_aux(float x) {
   return __uint_as_float(u);
 }
 
-static inline unsigned grid_for(int64_t n, int threads, int64_t cap = 148 * 16) {
+static inline unsigned grid_for(int64_t n, int threads, int64_t cap = 132 * 16) {
   int64_t g = (n + threads - 1) / threads;
   if (g < 1) g = 1;
   if (g > cap) g = cap;
@@ -320,9 +320,9 @@ void launch_delta_mean(const float* ssum, const float* shift, double n_total, do
 }
 
 // ------------------------------------------------------------------ exact Gram diagonal of a split slab
-// out[c] += sum_r (hi[r][c] + lo[r][c])^2 in fp64 (out must be zeroed).  The tensor core chops every product of an MMA step at
-// the accumulator's granularity, toward zero: entries whose products all have one sign -- the diagonal of S^T S -- lose
-// ~7.5e-8 of their value per step of the accumulation chain, zero-mean entries lose nothing (profiles/r2_trunc_probe.txt).
+// out[c] += sum_r (hi[r][c] + lo[r][c])^2 in fp64 (out must be zeroed).  The tensor core's fp32 accumulation does not round
+// every product to nearest: entries whose products all have one sign -- the diagonal of S^T S -- are biased along the
+// accumulation chain, zero-mean entries are not (tools/trunc_probe.py measures it).
 // The split-operand mode therefore takes the diagonal from this reduction instead of from the tensor core.
 template <class T2>
 __device__ __forceinline__ float2 pair_to_float2(T2 v);
@@ -692,7 +692,7 @@ void launch_max_abs_f32(const float* p, int64_t ld, int64_t rows, int cols, unsi
 }
 void launch_max_abs_f64(const double* p, int64_t n, unsigned* maxbits, cudaStream_t st) {
   if (n == 0) return;
-  max_abs_f64_kernel<<<grid_for(n, 256, 148 * 2), 256, 0, st>>>(p, n, maxbits);
+  max_abs_f64_kernel<<<grid_for(n, 256, 132 * 2), 256, 0, st>>>(p, n, maxbits);
 }
 void launch_pow2_scale(const unsigned* maxbits, float target, float* scale, cudaStream_t st) {
   pow2_scale_kernel<<<1, 1, 0, st>>>(maxbits, target, scale);

@@ -139,7 +139,7 @@ __global__ void final_b_finish_kernel(const double* __restrict__ jlm, const doub
 
 static unsigned grid1d(int64_t n, int threads = 256) {
   int64_t g = (n + threads - 1) / threads;
-  return static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(g, 1), 148 * 16));
+  return static_cast<unsigned>(std::min<int64_t>(std::max<int64_t>(g, 1), 132 * 16));
 }
 
 // ------------------------------------------------------------------------------------ fit

@@ -419,7 +419,7 @@ void prepare_generated_operands(Ctx& c, FeatSrc& out, int precision) {
                       static_cast<int>(out.X->cols), c.st);
   c.launches += 1;
   if ((want_f16 && c.proj_f16) || want_x2) {
-    // fp16 copies of X and W for the kind::f16 projection.  Each carries its own power-of-two scale (largest magnitude
+    // fp16 copies of X and W for the fp16 projection.  Each carries its own power-of-two scale (largest magnitude
     // mapped into [2048, 4096]), so the input units do not matter; the product of the two inverse scales is applied to the
     // fp32 accumulator in the epilogue.  Same 10-bit mantissa as the tf32 operands above.
     out.pscale.alloc(sizeof(float) * 8);  // [0] 1/(sx*sw)  [1] maxbits x  [2] maxbits w  [4,5] x {s, 1/s}  [6,7] w {s, 1/s}
@@ -512,9 +512,8 @@ static void tmap16_or_throw(CUtensorMap* m, const void* base, int64_t rows, int6
                                    " cols=" + std::to_string(cols) + " ld=" + std::to_string(ld)};
 }
 
-static void tmap_or_throw(CUtensorMap* m, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
-                          bool atom32 = false) {
-  const int r = make_tmap_2d(m, base, rows, cols, ld, box_rows, atom32);
+static void tmap_or_throw(CUtensorMap* m, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  const int r = make_tmap_2d(m, base, rows, cols, ld, box_rows);
   if (r != 0)
     throw KsError{KS_ERR_CUDA, "cuTensorMapEncodeTiled failed (" + std::to_string(r) + ") rows=" + std::to_string(rows) +
                                    " cols=" + std::to_string(cols) + " ld=" + std::to_string(ld)};
@@ -538,18 +537,18 @@ void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* s
     if (!src.proj_x2 || out16 || round_out) throw KsError{KS_ERR_INVALID, "split-operand slab requested without split operands"};
     kdepth = 3 * src.d_in;
     tmap16_or_throw(&k.tmA, static_cast<const uint16_t*>(src.x3.p) + row_begin * src.ldx3, rows, kdepth, src.ldx3, 64, 128, TMAP_SW128);
-    tmap16_or_throw(&k.tmB, static_cast<const uint16_t*>(src.w3.p) + c0 * src.ldw3, cols, kdepth, src.ldw3, 64, 256, TMAP_SW128);
+    tmap16_or_throw(&k.tmB, static_cast<const uint16_t*>(src.w3.p) + c0 * src.ldw3, cols, kdepth, src.ldw3, 64, 128, TMAP_SW128);
     k.f16 = 1;
     k.p.acc_scale_ptr = src.pscale.as<float>();
   } else if (out16 && src.proj16) {  // fp16 operands: 64 K-elements (128 B) per box row
     tmap16_or_throw(&k.tmA, static_cast<const uint16_t*>(src.xop16.p) + row_begin * src.X->ld, rows, src.d_in, src.X->ld, 64, 128,
                     TMAP_SW128);
-    tmap16_or_throw(&k.tmB, static_cast<const uint16_t*>(src.w16.p) + c0 * src.ldw, cols, src.d_in, src.ldw, 64, 256, TMAP_SW128);
+    tmap16_or_throw(&k.tmB, static_cast<const uint16_t*>(src.w16.p) + c0 * src.ldw, cols, src.d_in, src.ldw, 64, 128, TMAP_SW128);
     k.f16 = 1;
     k.p.acc_scale_ptr = src.pscale.as<float>();
   } else {
     tmap_or_throw(&k.tmA, src.xop.as<float>() + row_begin * src.X->ld, rows, src.d_in, src.X->ld, 128);
-    tmap_or_throw(&k.tmB, src.Wall + c0 * src.ldw, cols, src.d_in, src.ldw, 256);
+    tmap_or_throw(&k.tmB, src.Wall + c0 * src.ldw, cols, src.d_in, src.ldw, 128);
   }
   if (slab_lo && !x2) throw KsError{KS_ERR_INVALID, "a lo plane needs the split operands"};
   if (slab_lo) {  // the epilogue splits the unrounded value into the fp16 pair itself: no fp32 copy of the block, no second pass
@@ -570,7 +569,6 @@ void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* s
   k.p.flags = (round_out ? 0 : KM_FLAG_NO_ROUND) | (src.kind == 1 ? KM_FLAG_RECT : 0);
   k.p.rect_floor = src.rect_floor;
   k.epi = EPI_COS;
-  k.pair = 0;
   // the projection kernel is persistent (one CTA per SM for its whole duration); on the look-ahead stream leave a few SMs
   // free so that the critical chain's small kernels (NCCL all-reduce, triangular solves) can always be scheduled
   k.num_sms = (st == c.st2) ? std::max(1, c.num_sms - c.reserve_sms) : c.num_sms;
@@ -579,11 +577,11 @@ void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* s
   c.launches += 1;
 }
 
-const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, bool pair, int* num_tiles) {
-  std::vector<int> key = {b, kcols, with_g ? 1 : 0, with_c ? 1 : 0, pair ? 1 : 0};
+const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, int* num_tiles) {
+  std::vector<int> key = {b, kcols, with_g ? 1 : 0, with_c ? 1 : 0};
   auto it = c.tile_cache.find(key);
   std::vector<GramTile> t;
-  const int tm = pair ? 256 : 128, tn = pair ? 512 : 256;
+  const int tm = 128, tn = 128;
   const int mb = (b + tm - 1) / tm;
   if (with_g) {
     const int nbk = (b + tn - 1) / tn;
@@ -614,10 +612,8 @@ void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int 
   if (!st) st = c.st;
   GramLaunch g;
   int nt = 0;
-  g.pair = f16 ? 1 : c.gram_pair;
   g.f16 = f16 ? 1 : 0;
-  g.epi_multi = c.epi_multi;
-  g.tiles = gram_tiles(c, b, kcols, with_g, with_c, g.pair != 0, &nt);
+  g.tiles = gram_tiles(c, b, kcols, with_g, with_c, &nt);
   g.num_tiles = nt;
   const int stage_rows = f16 ? 64 : kGramStageRows;
   if (f16) {  // MN-major fp16 operands: 64-column (128 B) x 64-row boxes, plain 128 B swizzle
@@ -626,16 +622,15 @@ void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int 
     if (with_c) tmap16_or_throw(&g.tmB1, R, rows, kcols, ldr, 64, stage_rows, TMAP_SW128);
     else g.tmB1 = g.tmA;
   } else {
-    tmap_or_throw(&g.tmA, static_cast<const float*>(slab), rows, b, lds, kGramStageRows, true);
+    tmap_or_throw(&g.tmA, static_cast<const float*>(slab), rows, b, lds, kGramStageRows);
     g.tmB0 = g.tmA;
-    if (with_c) tmap_or_throw(&g.tmB1, static_cast<const float*>(R), rows, kcols, ldr, kGramStageRows, true);
+    if (with_c) tmap_or_throw(&g.tmB1, static_cast<const float*>(R), rows, kcols, ldr, kGramStageRows);
     else g.tmB1 = g.tmA;
   }
   g.rows = static_cast<int>(rows);
-  // Rows of the contraction per CTA (pair).  Every chunk ends in a reduce-add of its 256 x 512 partial tile, so long
-  // chunks mean less reduce traffic and fewer, longer CTAs next to the critical chain's kernels; short chunks keep enough
-  // CTAs per launch to balance 74 CTA pairs when the rows are sharded.  Measured in the config-3 fit (tools/ab_fit.py,
-  // fp16 operands, N = 1M): 4096 -> 660 ms, 8192 -> 655 ms, 16384 -> 639 ms, 32768 -> 650 ms.
+  // Rows of the contraction per CTA.  Every chunk ends in a reduce-add of its 128 x 128 partial tile, so long chunks mean
+  // less reduce traffic and fewer, longer CTAs next to the critical chain's kernels; short chunks keep enough CTAs per
+  // launch to balance the SMs when the rows are sharded (tools/ab_fit.py compares settings).
   int64_t chunk = chunk_rows > 0 ? chunk_rows : c.gram_chunk_rows;
   if (chunk <= 0) chunk = !f16 ? 4096 : rows >= 400000 ? 16384 : rows >= 200000 ? 8192 : 4096;
   chunk = std::max<int64_t>(stage_rows, chunk / stage_rows * stage_rows);
@@ -656,7 +651,6 @@ void launch_update(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, c
   if (rows <= 0 || k <= 0 || b <= 0) return;
   if (!st) st = c.st;
   KmLaunch u;
-  u.pair = f16 ? 1 : c.gram_pair;
   u.f16 = f16 ? 1 : 0;
   u.p.acc_scale_ptr = acc_scale_ptr;
   if (f16) {  // K-major fp16 operands: 64 K-elements (128 B) x 128 rows per box
@@ -664,7 +658,7 @@ void launch_update(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, c
     tmap16_or_throw(&u.tmB, bop, k, b, ldb, 64, 128, TMAP_SW128);
   } else {
     tmap_or_throw(&u.tmA, static_cast<const float*>(slab), rows, b, lds, 128);
-    tmap_or_throw(&u.tmB, static_cast<const float*>(bop), k, b, ldb, u.pair ? 128 : 256);
+    tmap_or_throw(&u.tmB, static_cast<const float*>(bop), k, b, ldb, 128);
   }
   tmap_or_throw(&u.tmOut, out, rows, k, ldo, 32);  // k valid columns: the store never touches columns >= k
   u.p.vec0 = cbias;
@@ -673,7 +667,7 @@ void launch_update(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, c
   u.p.M = static_cast<int>(rows);
   u.p.N = k;
   u.p.K = b;
-  u.p.flags = (reduce ? KM_FLAG_REDUCE : 0) | ((u.pair && c.epi_multi) ? KM_FLAG_EPI_MULTI : 0);
+  u.p.flags = reduce ? KM_FLAG_REDUCE : 0;
   u.epi = epi;
   u.num_sms = c.num_sms;
   KS_CUDA(launch_kmajor(u, st));
@@ -716,9 +710,8 @@ __global__ void sumsq_f64_kernel(const double* p, int64_t n, double* out) {
 //
 // pipeline 1 (default): ONE stream carries every tensor-core kernel in the order C(j), G(j+1), proj(j+2), update(j); the
 // solve and factor chains run on their own higher-priority streams and hide under G(j+1) + proj(j+2).  Two tensor
-// kernels never share the SMs: each is written to own an SM (one CTA, ~200 KB of shared memory, all of TMEM), so running
-// two at once only splits the machine, thrashes L2 and stretches both (round 1 measured 40.4 ms per block for 29.3 ms of
-// isolated tensor work with the two-stream arrangement, i.e. worse than running everything back to back).
+// kernels never share the SMs: each is written to own an SM (one CTA, ~200 KB of shared memory), so running two at once
+// only splits the machine, thrashes L2 and stretches both.
 // pipeline 0: the round-1 arrangement (residual chain on st, look-ahead tensor kernels on st2), kept for A/B runs.
 // Slabs, G and H are triple-buffered; cross-stream dependencies are CUDA events; no host synchronisation inside the loop.
 static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double lam, int64_t nf_opt,
@@ -803,20 +796,20 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
 
   // ---- operand modes
   // KS_PRECISION_F16: the slab, the residual operand and the increment operand are fp16 and the three big GEMMs run as
-  //   kind::f16 -- same 10-bit mantissa as tf32 at twice the MMA rate and half the slab bytes.  Only for generated cosine
+  //   fp16 MMA -- same 10-bit mantissa as tf32 at twice the MMA rate and half the slab bytes.  Only for generated cosine
   //   features (|value| <= 2: no range problem); the residual and the increments are scaled by device-chosen powers of two.
   //   Materialised feature matrices have arbitrary scale and keep the tf32 path.
   // KS_PRECISION_F16X2 (the parity mode): every MMA operand v is carried as hi + lo (hi = round(v), lo = round(v - hi): 21+
   //   significant bits) and every product keeps hi*hi + hi*lo + lo*hi, using the same kernels three times (the projection
-  //   once, on operands concatenated along K).  Generated features: fp16 pairs (kind::f16); materialised features: tf32
-  //   pairs (kind::tf32, no range limits).
+  //   once, on operands concatenated along K).  Generated features: fp16 pairs (fp16 MMA); materialised features: tf32
+  //   pairs (tf32 MMA, no range limits).
   // fp16 slabs only for cosine features (|value| <= 2); rectified linear features have the scale of their input
   const bool x2 = precision == KS_PRECISION_F16X2 && (src.F || src.proj_x2);
   const bool f16 = !src.F && src.kind == 0 && (precision == KS_PRECISION_F16 || x2);
   const size_t es = f16 ? 2 : 4;  // bytes per slab / operand element
-  const int64_t x2_chunk = c.split_chunk_rows;  // short accumulation chains: the tensor core's fp32 accumulate truncates (~2^-25 per MMA step)
+  const int64_t x2_chunk = c.split_chunk_rows;  // short accumulation chains: the tensor core's fp32 accumulate truncates
   // look-ahead of the residual-independent work (projection, G-Gram, factorisation) over the residual chain, in blocks.  With the
-  // rows sharded over GPUs the Cholesky of block t+1 (2.5 ms alone, more next to tensor kernels) sits in a dependency cycle
+  // rows sharded over GPUs the Cholesky of block t+1 (slower next to tensor kernels than alone) sits in a dependency cycle
   // G(t+1) -> factor(t+1) -> solve(t+1) -> update(t+1) -> ... -> G(t+1+LA): a deeper look-ahead spreads it over more blocks.
   const int LA = (serial && (c.pipeline == 1 || c.pipeline == 4)) ? (c.lookahead > 0 ? c.lookahead : (c.world > 1 ? 2 : 1)) : 1;
   const int NBUF = LA + 2;
@@ -1406,7 +1399,8 @@ KS_API int32_t ks_ctx_create(int32_t device_id, int32_t rank, int32_t world_size
     KS_CUDA(cudaSetDevice(device_id));
     cudaDeviceProp prop;
     KS_CUDA(cudaGetDeviceProperties(&prop, device_id));
-    if (prop.major != 10) throw KsError{KS_ERR_NO_DEVICE, std::string("device is sm_") + std::to_string(prop.major) + std::to_string(prop.minor) + "; this library contains sm_100a code only"};
+    if (prop.major != 9 || prop.minor != 0)
+      throw KsError{KS_ERR_NO_DEVICE, std::string("device is sm_") + std::to_string(prop.major) + std::to_string(prop.minor) + "; this library contains sm_90a code only"};
     auto c = std::make_unique<Ctx>();
     c->device = device_id;
     c->rank = rank;
@@ -1422,8 +1416,6 @@ KS_API int32_t ks_ctx_create(int32_t device_id, int32_t rank, int32_t world_size
       const long v = atol(e);
       if (v >= kGramStageRows) c->gram_chunk_rows = v;
     }
-    if (const char* e = getenv("KS_GRAM_PAIR")) c->gram_pair = atoi(e) != 0;
-    if (const char* e = getenv("KS_EPI_MULTI")) c->epi_multi = atoi(e) != 0;
     if (const char* e = getenv("KS_SHARD_SOLVE")) c->shard_solve = atoi(e) != 0;
     if (const char* e = getenv("KS_PROJ_F16")) c->proj_f16 = atoi(e) != 0;
     if (const char* e = getenv("KS_PRECISION"))
@@ -1530,13 +1522,11 @@ KS_API int32_t ks_ctx_set_option(int64_t ctx, const char* name, int64_t value) {
     if (n == "gram_chunk_rows" && (value == 0 || value >= kGramStageRows)) c.gram_chunk_rows = value;
     else if (n == "split_chunk_rows" && value >= kGramStageRows && value % kGramStageRows == 0) c.split_chunk_rows = value;
     else if (n == "sample_rows" && value >= 1) c.sample_rows = value;
-    else if (n == "gram_pair") c.gram_pair = value != 0;
-    else if (n == "epi_multi") c.epi_multi = value != 0;
     else if (n == "shard_solve") c.shard_solve = value != 0;
     else if (n == "proj_f16") c.proj_f16 = value != 0;
     else if (n == "precision" && (value == KS_PRECISION_TF32 || value == KS_PRECISION_F16 || value == KS_PRECISION_F16X2)) c.precision = static_cast<int>(value);
     else if (n == "custom_solve" && value >= -1 && value <= 1) c.custom_solve = static_cast<int>(value);
-    else if (n == "reserve_sms" && value >= 0 && value < 148) c.reserve_sms = static_cast<int>(value);
+    else if (n == "reserve_sms" && value >= 0 && value < c.num_sms) c.reserve_sms = static_cast<int>(value);
     else if (n == "pipeline" && value >= 0 && value <= 4) c.pipeline = static_cast<int>(value);
     else if (n == "dyn_tiles") c.dyn_tiles = value != 0;
     else if (n == "lookahead" && value >= 0 && value <= 6) c.lookahead = static_cast<int>(value);
@@ -1879,9 +1869,8 @@ KS_API int32_t ks_convolver_apply(int64_t ctx, int64_t conv, int64_t images, int
       KmLaunch k;
       const int64_t m_rows = ni * ppi;
       tmap16_or_throw(&k.tmA, patches.p, m_rows, kdepth, ldp, 64, 128, TMAP_SW128);
-      tmap16_or_throw(&k.tmB, x2 ? cv.w3.p : cv.w16.p, cv.n_filters, kdepth, ldp, 64, 256, TMAP_SW128);
+      tmap16_or_throw(&k.tmB, x2 ? cv.w3.p : cv.w16.p, cv.n_filters, kdepth, ldp, 64, 128, TMAP_SW128);
       k.f16 = 1;
-      k.pair = 0;
       k.p.acc_scale_ptr = cv.wscale.as<float>() + 3;      // 2^-e of the filter scale
       k.p.M = static_cast<int>(m_rows);
       k.p.N = cv.n_filters;
@@ -2258,7 +2247,7 @@ KS_API int32_t ks_last_fit_stats_json(int64_t ctx, char* buf, int64_t buflen) {
 }
 
 // ---------------------------------------------------------------- debug / micro-benchmarks
-// With the context option precision = KS_PRECISION_F16 the operands are first converted to fp16 and the kind::f16 kernel runs.
+// With the context option precision = KS_PRECISION_F16 the operands are first converted to fp16 and the fp16 kernel runs.
 struct DebugGramOps {
   DevBuf a16, b16;
   const void* A = nullptr;

@@ -153,7 +153,7 @@ enum Phase { PH_FEATURIZE = 0, PH_GRAM, PH_ALLREDUCE, PH_SOLVE, PH_UPDATE, PH_OT
 
 struct Ctx {
   int device = 0, rank = 0, world = 1;
-  int num_sms = 148;
+  int num_sms = 132;
   // Stream roles of the pipelined fit (engine.cu::fit_blockls), pipeline = 1 (default):
   //   st  (highest priority) solve chain: all-reduce of C, rhs assembly, triangular solves, operand packing
   //   st2 (lowest priority)  ALL tensor-core kernels in one order: C(j), G(j+1), proj(j+2), update(j) -- never two at once
@@ -194,20 +194,15 @@ struct Ctx {
   std::string err;
   std::string stats_json;
   int64_t launches = 0;
-  int64_t gram_chunk_rows = 0;  // rows of the contraction per Gram CTA (pair); 0 = chosen from the local row count (engine.cu)
+  int64_t gram_chunk_rows = 0;  // rows of the contraction per Gram CTA; 0 = chosen from the local row count (engine.cu)
   int64_t split_chunk_rows = 4096;  // the same in the parity mode: short accumulation chains (the tensor core chops products at the accumulator granularity)
-  int gram_pair = 1;  // CTA-pair (cta_group::2) Gram kernel
-  int epi_multi = 1;  // CTA-pair kernels: 8 rotating epilogue staging buffers per warp (0: one buffer, store-and-wait)
   int proj_f16 = 1;   // fp16 mode: the projection GEMM X W^T runs with fp16 operands too (0: tf32 operands, fp16 slab)
   int precision = KS_PRECISION_F16X2;  // what KS_PRECISION_DEFAULT resolves to: the split-operand parity mode
   int reserve_sms = 8; // SMs the persistent look-ahead kernel leaves to the critical chain
   int custom_solve = -1; // triangular solves of the critical chain: 0 = cusolverDnDpotrs, 1 = the library's DMMA kernel
                          // (solve_kernels.cu: one launch, co-resident with the look-ahead Gram CTAs), -1 = automatic: the DMMA
                          // kernel when the rank solves <= 512 right-hand sides (the column-sharded multi-GPU solve, where its
-                         // CTA clusters cut the latency: 1.6 - 2.7 ms for 125 - 500 columns vs 2.6 - 3.0 ms for potrs alone and
-                         // ~10 ms for potrs next to the tensor kernels), potrs otherwise.  Measured (profiles/README.md, round 2):
-                         // N = 1, 1000 columns: the kernel hides under the Gram (11.9 vs 18.7 ms) but slows that Gram from 13.0
-                         // to 17.1 ms -- a wash; N = 2, 500 columns: 341.9 vs 352.9 ms per fit.
+                         // CTA clusters cut the latency of the substitution), potrs otherwise.
   int64_t sample_rows = 16384;
   int64_t next_id = 1;
   std::unordered_map<int64_t, std::unique_ptr<Matrix>> matrices;
@@ -282,7 +277,7 @@ void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* s
                   int64_t row_begin, int64_t rows, bool round_out = true, float* colsum = nullptr, cudaStream_t st = nullptr,
                   bool out16 = false, bool x2 = false,  // x2: unrounded slab from the K-concatenated split operands: fp32, or
                   void* slab_lo = nullptr);             // (slab_lo given) the fp16 pair hi -> slab, lo -> slab_lo written by the epilogue
-const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, bool pair, int* num_tiles);
+const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, int* num_tiles);
 // f16: slab and R are fp16 matrices (leading dimensions in elements); G / C stay fp32
 void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, const void* R, int64_t ldr, int kcols,
                        float* G, int ldg, float* C, int ldc, bool with_g, bool with_c, cudaStream_t st = nullptr,

@@ -13,23 +13,21 @@ enum { EPI_COS = 0, EPI_UPDATE = 1, EPI_APPLY = 2, EPI_POOL = 3 };
 
 struct GramTile {
   int m_blk;  // 128-wide block of A's columns
-  int n_blk;  // BN-wide block of B's columns
+  int n_blk;  // 128-wide block of B's columns
   int which;  // 0: B = tmB0 -> out0,  1: B = tmB1 -> out1
   int pad;
 };
 struct GramLaunch {
-  CUtensorMap tmA, tmB0, tmB1;   // operands: box {32, kGramStageRows}, SWIZZLE_128B_ATOM_32B
+  CUtensorMap tmA, tmB0, tmB1;   // operands: tf32 box {32, kGramStageRows}, fp16 box {64, 64}; SWIZZLE_128B
   CUtensorMap tmOut0, tmOut1;    // outputs:  box {32, 32}, SWIZZLE_128B; dims clip the reduce-add at the matrix edge
   const GramTile* tiles;         // device
   int num_tiles;
   int rows;        // contraction length (rows of A and B)
   int chunk_rows;  // split of the contraction across CTAs (multiple of kGramStageRows)
   int n_valid0, n_valid1;  // valid output columns per target (whole 32-column chunks beyond are skipped)
-  int pair;                // 1: CTA-pair kernel (tiles are 256 x 512), 0: single-CTA kernel (tiles are 128 x 256)
-  int epi_multi = 1;       // CTA-pair kernel: rotate the epilogue through 8 staging buffers per warp (idle stage memory)
-  int f16 = 0;             // 1: operands are fp16 (kind::f16, CTA-pair kernel, 64-row stages), 0: tf32
+  int f16 = 0;             // 1: operands are fp16 (wgmma, 64-row stages), 0: tf32 (mma.sync, 32-row stages)
 };
-enum { KM_FLAG_NO_ROUND = 1, KM_FLAG_REDUCE = 2, KM_FLAG_EPI_MULTI = 4, KM_FLAG_RECT = 8 };
+enum { KM_FLAG_NO_ROUND = 1, KM_FLAG_REDUCE = 2, KM_FLAG_RECT = 8 };
 struct KmParams {
   const float* vec0;  // EPI_COS: bias (KM_FLAG_RECT: alpha);  EPI_UPDATE / EPI_APPLY: per-column constant
   float rect_floor = 0.f;   // KM_FLAG_RECT: the feature is max(rect_floor, acc - alpha) instead of cos(acc + bias)
@@ -49,20 +47,19 @@ struct KmParams {
   int flags;  // KM_FLAG_NO_ROUND: EPI_COS keeps fp32;  KM_FLAG_REDUCE: add into the output instead of overwriting it
 };
 struct KmLaunch {
-  CUtensorMap tmA, tmB;  // operands: box {32, 128} / {32, 256}, SWIZZLE_128B
+  CUtensorMap tmA, tmB;  // operands: box {32, 128} (tf32) / {64, 128} (fp16), SWIZZLE_128B
   CUtensorMap tmOut;     // output: box {32, 32}, SWIZZLE_128B
   CUtensorMap tmOut2;    // out16 == 2 only: the lo plane (same geometry as tmOut)
   KmParams p;
   int epi;
   int num_sms;
-  int pair;  // 1: CTA-pair kernel (EPI_UPDATE / EPI_APPLY; tmB box is {32, 128}), 0: single-CTA persistent kernel
-  int f16 = 0;   // 1: fp16 operands (EPI_UPDATE / EPI_APPLY on CTA pairs; boxes are {64, 128} fp16)
+  int f16 = 0;   // 1: fp16 operands
   int out16 = 0; // EPI_COS: 1 = the slab is written as fp16 (tmOut: {32, 32} fp16 boxes, no swizzle); 2 = as the fp16 pair hi + lo
                  // of the unrounded value (tmOut, tmOut2)
 };
 
-int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows, bool atom32 = false);
-enum { TMAP_SW128 = 0, TMAP_SW128_ATOM32 = 1, TMAP_NONE = 2 };
+int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows);
+enum { TMAP_SW128 = 0, TMAP_NONE = 2 };
 int make_tmap_any(CUtensorMap* out, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows,
                   int elem_bytes, int swizzle);
 cudaError_t launch_gram(const GramLaunch& g, cudaStream_t st);

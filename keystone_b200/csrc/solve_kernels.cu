@@ -2,13 +2,12 @@
 //
 // Replaces cusolverDnDpotrs on the critical chain of the block solver (the reference's `\` on the driver,
 // K/nodes/learning/BlockWeightedLeastSquares.scala:272, mlmatrix NormalEquations for BlockLS).  cuSOLVER runs the two
-// triangular solves as ~230 small dependent kernels: 4.4 ms alone, but 26 ms when they share the GPU with the tensor-core
-// kernels of the look-ahead (profiles/README.md, round 2: every one of those launches waits for SMs that 140-microsecond Gram
-// CTAs or the persistent projection kernel are holding) -- the critical path of the whole fit.  This kernel is built to run
-// BESIDE them instead:
+// triangular solves as ~230 small dependent kernels; when they share the GPU with the tensor-core kernels of the look-ahead,
+// every one of those launches waits for SMs that Gram CTAs or the persistent projection kernel are holding -- on the critical
+// path of the whole fit.  This kernel is built to run BESIDE them instead:
 //   * one launch; a CTA owns NC right-hand sides and performs the complete forward and backward substitution for them, so
 //     there is no inter-CTA dependency and no grid synchronisation;
-//   * no shared-memory tiles in the bulk loops and 10 KB in total: it fits next to a 209 KB Gram CTA on the same SM
+//   * no shared-memory tiles in the bulk loops and 10 KB in total: it fits next to a ~196 KB Gram CTA on the same SM
 //     (registers and thread slots are free there), so its CTAs become resident at once instead of queueing for an SM;
 //   * all bulk arithmetic is DMMA (mma.sync.m8n8k4.f64) with operand fragments loaded straight from L2 in fully used
 //     32 / 64 B sectors; the in-tile substitutions are products with the pre-inverted 64 x 64 diagonal tiles (tri_inv_tiles,
@@ -318,9 +317,9 @@ cudaError_t launch_chol_solve(const double* L, const double* Dinv, int n, double
   // column-sharded multi-GPU solve) 8 per CTA keep more SMs busy
   static const int forced_nc = getenv("KS_SOLVE_NC") ? atoi(getenv("KS_SOLVE_NC")) : 0;   // A/B override (8 or 16)
   static const int forced_cl = getenv("KS_SOLVE_CLUSTER") ? atoi(getenv("KS_SOLVE_CLUSTER")) : -1;   // -1: chosen from k; 0 / 1: off
-  // few right-hand sides: clusters of CTAs share one group of 8 columns, so that ~128 CTAs work whatever k is
+  // few right-hand sides: clusters of CTAs share one group of 8 columns, so that up to one CTA per SM (132) works whatever k is
   const int groups = (k + 7) / 8;
-  int cl = forced_cl >= 0 ? forced_cl : (groups <= 18 ? 8 : groups <= 37 ? 4 : groups <= 74 ? 2 : 1);
+  int cl = forced_cl >= 0 ? forced_cl : (groups <= 16 ? 8 : groups <= 33 ? 4 : groups <= 66 ? 2 : 1);
   if (cl > 1) {
     if (cl != 2 && cl != 4 && cl != 8) return cudaErrorInvalidValue;
     cudaLaunchConfig_t cfg = {};
@@ -337,7 +336,7 @@ cudaError_t launch_chol_solve(const double* L, const double* Dinv, int n, double
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, chol_solve_cluster_kernel, L, Dinv, n, B, k);
   }
-  const bool nc16 = forced_nc ? forced_nc == 16 : k > 8 * 148;
+  const bool nc16 = forced_nc ? forced_nc == 16 : k > 8 * 132;
   if (nc16) chol_solve_kernel<16><<<(k + 15) / 16, 256, 0, st>>>(L, Dinv, n, B, k);
   else chol_solve_kernel<8><<<(k + 7) / 8, 256, 0, st>>>(L, Dinv, n, B, k);
   return cudaGetLastError();

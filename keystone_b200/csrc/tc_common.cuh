@@ -1,6 +1,6 @@
-// Blackwell (sm_100a) device-side primitives shared by the tensor-core kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the
-// shared-memory + instruction descriptors for kind::tf32.  Inline PTX only.
+// Hopper (sm_90a) device-side primitives shared by the tensor-core kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait) with its
+// shared-memory descriptors, and the warp-level tf32 mma.sync.  Inline PTX only.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -10,7 +10,7 @@
 namespace ks {
 
 // Error flag written (and the kernel trapped) when a barrier wait exceeds its budget:
-// a descriptor / pipeline bug then fails the launch instead of hanging the GPU box.
+// a descriptor / pipeline bug then fails the launch instead of hanging the GPU.
 __device__ unsigned int g_wait_timeout_flag = 0;
 
 static constexpr unsigned long long kWaitBudgetCycles = 6000000000ull;  // ~3 s at 2 GHz
@@ -29,6 +29,11 @@ __device__ __forceinline__ bool elect_one() {
       "}\n"
       : "=r"(pred));
   return pred != 0;
+}
+
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ---------------------------------------------------------------- mbarrier
@@ -103,8 +108,6 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-// at most 7 of this thread's bulk groups may still be reading their shared-memory source (8 rotating staging buffers)
-__device__ __forceinline__ void bulk_wait_read7() { asm volatile("cp.async.bulk.wait_group.read 7;" ::: "memory"); }
 
 // Epilogue staging: thread `lane` owns row `lane` of a 32 x 32 fp32 chunk (128 B per row) and writes it into a
 // 4 KB, 1024 B-aligned shared buffer in the 128 B-swizzled order a {32, 32} SWIZZLE_128B tensor map expects
@@ -116,161 +119,71 @@ __device__ __forceinline__ void stage_row_sw128(uint8_t* buf, int lane, const fl
     *reinterpret_cast<float4*>(row + ((c ^ (lane & 7)) << 4)) = make_float4(o[4 * c], o[4 * c + 1], o[4 * c + 2], o[4 * c + 3]);
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_out, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_out)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32, issued by ONE thread for the CTA.
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::f16 (fp16 operands, fp32 accumulate): twice the tf32 rate with the same 10-bit mantissa; K = 16 per instruction.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued MMAs of this thread arrive on the mbarrier when complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp gets lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load issued by either CTA of a pair; the transaction bytes are credited to the LEADER CTA's mbarrier (same
-// shared offset, peer bit 24 of the shared::cluster address cleared), which is the only barrier the MMA issuer waits on.
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_out, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_out)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// M = 256 MMA across the CTA pair (each CTA supplies its 128 rows of A and its half of B's N columns); leader issues.
-__device__ __forceinline__ void umma_tf32_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-template <bool F16>
-__device__ __forceinline__ void umma_pair(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  if (F16) umma_f16_pair(d, a, b, idesc, acc);
-  else umma_tf32_pair(d, a, b, idesc, acc);
-}
-// completion of the leader's MMAs arrives on the barrier at the same shared offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(static_cast<uint16_t>(3))
-               : "memory");
-}
-
-// ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (64-bit).  Fields (PTX ISA, tcgen05 matrix descriptor):
+// ---------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor (64-bit, sm_90).  Fields (PTX ISA, warpgroup matrix descriptor):
 //   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1 (sm_100)
-//   [49,52) base offset (0: tiles are 1024 B aligned)   [61,64) swizzle: 2 = 128 B
-//           1 = 128 B swizzle with 32 B atoms (the only layout accepted for MN-major tf32 operands)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout_type) {
+//   [32,46) stride-dim byte offset >> 4   [49,52) base offset (0: tiles are 1024 B aligned)   [62,64) swizzle: 1 = 128 B
+// K-major 128 B swizzle: rows of 128 B, 8-row groups SBO apart (LBO unused).  MN-major 128 B swizzle: 64 fp16 MN elements per
+// 128 B row, one K index per row; 64-wide MN blocks are LBO apart, 8-row K groups SBO apart.
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;
-  d |= static_cast<uint64_t>(layout_type & 7) << 61;
+  d |= 1ull << 62;
   return d;
 }
-static constexpr uint32_t kLayoutSw128 = 2;       // K-major operands: Swizzle<3,4,3> (16 B chunks ^ row % 8)
-static constexpr uint32_t kLayoutSw128Base32 = 1; // MN-major tf32: Swizzle<2,5,2> (32 B chunks ^ row % 4), 4-row K groups
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return make_smem_desc(saddr, lbo_bytes, sbo_bytes, kLayoutSw128);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads or writes of the accumulator registers across a wgmma fence / wait
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// Instruction descriptor, kind::tf32, fp32 accumulate.
-//   [4,6) D fmt: 1 = f32   [7,10) A fmt: 2 = tf32   [10,13) B fmt: 2 = tf32
-//   [15] A major (0 = K, 1 = MN)   [16] B major   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_tf32(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+
+#define KS_WG_D64                                                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, " \
+  "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "  \
+  "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define KS_WG_D64_OPS(d)                                                                                                      \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),     \
+      "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),    \
+      "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),    \
+      "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),    \
+      "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),    \
+      "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),    \
+      "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+
+// D[64 x 128] += A[64 x 16] B[16 x 128], fp16 operands from shared memory, fp32 accumulate, issued by the whole warpgroup.
+// TA / TB = 1: the operand is MN-major (the Gram's row-major slabs); 0: K-major.
+// accumulate = 0: D = A B.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " KS_WG_D64 ", %64, %65, p, 1, 1, %67, %68;\n\t}\n"
+      : KS_WG_D64_OPS(d)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
 }
-// kind::f16 with fp16 operands: A/B format field 0
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// D[64 x 128] += A[64 x 8] B[8 x 128], tf32 operands (fp32 containers) from shared memory; both operands K-major.
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " KS_WG_D64 ", %64, %65, p, 1, 1;\n\t}\n"
+      : KS_WG_D64_OPS(d)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// Warp-level D[16 x 8] += A[16 x 8] B[8 x 8], tf32 (operands already tf32-rounded in fp32 containers).  wgmma takes tf32
+// operands only K-major; the Gram's tf32 operands are MN-major, so its kernel builds these fragments itself.
+__device__ __forceinline__ void mma_tf32_16x8x8(float* d, const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
 // Round-to-nearest(-away) fp32 -> tf32 kept in an fp32 container: the MMA then sees exactly

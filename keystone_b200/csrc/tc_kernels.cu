@@ -1,4 +1,4 @@
-// Tensor-core kernels of the block least-squares hot path (sm_100a, tcgen05 + TMA + TMEM).
+// Tensor-core kernels of the block least-squares hot path (sm_90a: TMA + mbarrier pipelines feeding wgmma).
 //
 //   gram_tn_kernel    D[M x N] += A^T B over a chunk of rows, A [rows x M] and B [rows x N] both
 //                     row-major (contraction over the slow axis => both operands MN-major).
@@ -6,14 +6,18 @@
 //                     (K/nodes/learning/BlockWeightedLeastSquares.scala:212-214 and the mlmatrix
 //                     NormalEquations called from K/nodes/learning/BlockLinearMapper.scala:236-239).
 //   gemm_kmajor_kernel D[M x N] = A B^T, A [M x K] and B [N x K] row-major (K-major operands),
-//                     persistent, TMEM double-buffered, with fused epilogues:
+//                     persistent, with fused epilogues:
 //                       EPI_COS     out  = tf32(cos(acc + bias) - shift)     (CosineRandomFeatures.scala:30-32)
 //                       EPI_UPDATE  R   += -acc + cbias                      (BlockWeightedLeastSquares.scala:287-290)
 //                       EPI_APPLY   Y [+]= acc + cbias                       (BlockLinearMapper.scala:55-70)
+//                       EPI_POOL    Convolver -> SymmetricRectifier -> sum Pooler (Convolver.scala, Pooler.scala)
 //
-// Every epilogue goes TMEM -> registers -> 128 B-swizzled shared staging -> TMA store / TMA reduce-add, so global
-// memory only ever sees full 128 B rows (the first version stored 16 B per row per lane: 32 wavefronts per warp
-// instruction, which made the cosine epilogue 3x longer than its MMAs -- profiles/README.md).
+// Both kernels are 128 x 128 output tiles on 384 threads: warpgroup 0 issues the TMA loads of a 4-stage mbarrier ring,
+// warpgroups 1 and 2 each own 64 output rows (one m64n128 wgmma accumulator, 64 fp32 registers per thread) and run the
+// epilogue.  The accumulator goes registers -> shared memory (transposed so that lane i holds row i of a 32 x 32 chunk) ->
+// epilogue math -> 128 B-swizzled staging -> TMA store / TMA reduce-add, so global memory only sees full 128 B rows.
+// wgmma accepts tf32 operands only K-major, so the tf32 Gram (MN-major) builds warp-level mma.sync fragments from the same
+// TMA-filled stages instead.
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -21,338 +25,257 @@
 
 namespace ks {
 
-__host__ __device__ constexpr uint32_t tmem_cols_for(int n) { return n <= 32 ? 32u : n <= 64 ? 64u : n <= 128 ? 128u : n <= 256 ? 256u : 512u; }
+static constexpr int kThreads = 384;
+static constexpr int kTileM = 128, kTileN = 128;
+static constexpr int kStages = 4;
+static constexpr int kRawLd = 65;  // odd row pitch: lane i reading row i of the transpose buffer hits bank (i + col) % 32
+static constexpr int kRawBytes = 2 * 64 * kRawLd * 4;   // one 64 x 64 slab per consumer warpgroup
+static constexpr int kStagingBytes = 8 * 4096;          // one 32 x 32 fp32 chunk per consumer warp
+static constexpr int kVecBytes = 8 * 64 * 4;            // per-warp copies of 32 columns of vec0 and vec1
+static constexpr int kEpiBytes = kStagingBytes + kRawBytes + kVecBytes;
+static constexpr int kStageBytes = 32768;               // A and B tiles of one stage (128 x 128 B each)
+static constexpr int kSmemBytes = kStages * kStageBytes + kEpiBytes + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(kSmemBytes <= 227 * 1024, "shared memory per block");
+
+struct SmemLayout {
+  uint8_t* stages;
+  uint8_t* staging;  // 8 x 4 KB, 1024 B aligned
+  float* raw;        // 2 x [64][kRawLd]
+  float* vec;        // 8 x 64
+  uint64_t* full_bar;
+  uint64_t* empty_bar;
+  uint64_t* ring_bar;  // [8]
+  int* tile_ring;      // [8]
+};
+__device__ __forceinline__ SmemLayout carve_smem(uint8_t* smem_raw) {
+  SmemLayout L;
+  L.stages = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  L.staging = L.stages + kStages * kStageBytes;
+  L.raw = reinterpret_cast<float*>(L.staging + kStagingBytes);
+  L.vec = L.raw + 2 * 64 * kRawLd;
+  L.full_bar = reinterpret_cast<uint64_t*>(L.vec + 8 * 64);
+  L.empty_bar = L.full_bar + kStages;
+  L.ring_bar = L.empty_bar + kStages;
+  L.tile_ring = reinterpret_cast<int*>(L.ring_bar + 8);
+  return L;
+}
+
+// Accumulator of one warpgroup (m64n128 wgmma layout: register 4j + e of thread (warp w, lane l) is row 16w + l/4 + 8(e/2),
+// column 8j + 2(l%4) + e%2) -> columns [64 slab, +64) of the warpgroup's transpose buffer.
+__device__ __forceinline__ void wgmma_acc_to_raw(const float (&acc)[64], float* raw, int slab, int w, int lane) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int r = 16 * w + (lane >> 2) + 8 * (e >> 1);
+      const int c = 8 * jj + 2 * (lane & 3) + (e & 1);
+      raw[r * kRawLd + c] = acc[4 * (8 * slab + jj) + e];
+    }
+}
+
+// Epilogue walk shared by both kernels.  For each 64-column slab the warpgroup's accumulator goes through the transpose
+// buffer; warp w then holds rows 32 (w % 2) + lane and columns 32 (w / 2) + i of the slab as o[i] and calls
+// chunk(o, slab, row offset in the warpgroup, column offset in the tile).
+template <typename ToRaw, typename Chunk>
+__device__ __forceinline__ void epilogue_slabs(float* raw, int g, int w, int lane, ToRaw to_raw, Chunk chunk) {
+#pragma unroll  // constant slab: the accumulator registers are indexed statically
+  for (int slab = 0; slab < kTileN / 64; ++slab) {
+    to_raw(raw, slab);
+    named_bar_sync(1 + g, 128);
+    float o[32];
+    const float* src = raw + (32 * (w & 1) + lane) * kRawLd + 32 * (w >> 1);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = src[i];
+    named_bar_sync(1 + g, 128);  // the buffer is free for the next slab
+    chunk(o, slab, 32 * (w & 1), slab * 64 + 32 * (w >> 1));
+  }
+}
 
 // =====================================================================================
 // Gram / A^T B kernel (MN-major operands, split over row chunks, TMA reduce-add epilogue)
 // =====================================================================================
-static constexpr int kGramThreads = 192;  // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2-5: epilogue
-
-template <int BN, int SR, int STAGES>
+// F16: fp16 operands, 64-column (128 B) x 64-row TMA boxes, wgmma with both operands MN-major (K = 16 per instruction);
+// tf32: fp32 containers, 32-column x 32-row boxes, mma.sync m16n8k8 fragments (K = 8).  Either way a stage holds the 128
+// columns of A and of B for SR rows of the contraction: 32 KB.
+template <bool F16>
 struct GramCfg {
-  static constexpr int BM = 128;
-  static constexpr int A_BYTES = BM * SR * 4;
-  static constexpr int B_BYTES = BN * SR * 4;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BOX_BYTES = SR * 128;  // one TMA box: 32 floats (128 B) x SR rows
-  static constexpr int STAGING_BYTES = 4 * 4096;  // one 32 x 32 fp32 chunk per epilogue warp
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int SR = F16 ? 64 : 32;       // rows (K) per stage
+  static constexpr int CW = F16 ? 64 : 32;       // columns per TMA box (128 B)
+  static constexpr int NBOX = kTileM / CW;       // boxes per 128 operand columns
+  static constexpr int BOX_BYTES = SR * 128;
+  static constexpr int A_BYTES = NBOX * BOX_BYTES;
+  static_assert(2 * A_BYTES == kStageBytes, "stage size");
 };
 
-template <int BN, int SR, int STAGES>
-__global__ void __launch_bounds__(kGramThreads, 1)
+// tf32 element (column c, row r) of one MN-major operand tile: 32-column boxes of SR rows, 128 B swizzle
+template <int BOX_BYTES>
+__device__ __forceinline__ uint32_t ld_mn_tf32(const uint8_t* tile, int c, int r) {
+  return *reinterpret_cast<const uint32_t*>(tile + (c >> 5) * BOX_BYTES + r * 128 + (((((c & 31) >> 2) ^ (r & 7))) << 4) +
+                                            ((c & 3) << 2));
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(kThreads, 1)
 gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
                const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmOut0,
                const __grid_constant__ CUtensorMap tmOut1, const GramTile* __restrict__ tiles, int num_tiles, int rows,
                int chunk_rows, int n_valid0, int n_valid1) {
-  using Cfg = GramCfg<BN, SR, STAGES>;
+  using Cfg = GramCfg<F16>;
+  constexpr int SR = Cfg::SR;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+  const SmemLayout L = carve_smem(smem_raw);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
   const GramTile tile = tiles[blockIdx.x % num_tiles];
   const int chunk = blockIdx.x / num_tiles;
   const int row0 = chunk * chunk_rows;
   const int nrows = min(chunk_rows, rows - row0);
   const int ksteps = (nrows + SR - 1) / SR;
-  const int m0 = tile.m_blk * Cfg::BM;
-  const int n0 = tile.n_blk * BN;
-  const CUtensorMap* tmB = tile.which ? &tmB1 : &tmB0;
-  const CUtensorMap* tmOut = tile.which ? &tmOut1 : &tmOut0;
-  constexpr uint32_t kTmemCols = tmem_cols_for(BN);
-
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(tmB);
-    tma_prefetch_desc(tmOut);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&empty_bar[s], 1);
-      }
-      mbar_init(tmem_full_bar, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const int s = ks % STAGES;
-        const uint32_t ph = (ks / STAGES) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-        uint8_t* sA = smem + s * Cfg::STAGE_BYTES;
-        uint8_t* sB = sA + Cfg::A_BYTES;
-        const int r = row0 + ks * SR;
-#pragma unroll
-        for (int i = 0; i < Cfg::BM / 32; ++i) tma_load_2d(sA + i * Cfg::BOX_BYTES, &tmA, &full_bar[s], m0 + 32 * i, r);
-#pragma unroll
-        for (int i = 0; i < BN / 32; ++i) tma_load_2d(sB + i * Cfg::BOX_BYTES, tmB, &full_bar[s], n0 + 32 * i, r);
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc_tf32(Cfg::BM, BN, 1, 1);
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const int s = ks % STAGES;
-        const uint32_t ph = (ks / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t sA = smem_u32(smem + s * Cfg::STAGE_BYTES);
-        const uint32_t sB = sA + Cfg::A_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < SR / 8; ++kk) {
-          // MN-major tf32 => SWIZZLE_128B_BASE32B: 32-float MN chunks are BOX_BYTES apart (LBO), the two 4-row
-          // K groups of one K=8 MMA are 512 B apart (SBO); consecutive MMAs advance 8 rows = 1024 B.
-          const uint64_t ad = make_smem_desc(sA + kk * 1024, Cfg::BOX_BYTES, 512, kLayoutSw128Base32);
-          const uint64_t bd = make_smem_desc(sB + kk * 1024, Cfg::BOX_BYTES, 512, kLayoutSw128Base32);
-          umma_tf32(tmem_base, ad, bd, idesc, (ks | kk) != 0);
-        }
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(tmem_full_bar);
-    }
-  } else {
-    // epilogue: warp w owns TMEM lanes [32*(w&3), +32) == output rows m0 + 32*(w&3) + lane.  The partial tile is
-    // added to the fp32 output with one TMA reduce-add per 32 x 32 chunk (clipped at the matrix edge by the map).
-    const int q = warp & 3;
-    const int n_valid = tile.which ? n_valid1 : n_valid0;
-    uint8_t* buf = staging + (warp - 2) * 4096;
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      if (n0 + c0 >= n_valid) break;  // warp-uniform
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c0, v);
-      tmem_ld_wait();
-      float o[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(v[i]);
-      if (lane == 0) bulk_wait_read0();  // previous chunk's reduce has finished reading the staging buffer
-      __syncwarp();
-      stage_row_sw128(buf, lane, o);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        tma_reduce_add_2d(tmOut, buf, n0 + c0, m0 + q * 32);
-        bulk_commit();
-      }
-    }
-    if (lane == 0) bulk_wait0();
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-}
-
-// =====================================================================================
-// Gram / A^T B kernel on CTA pairs (cta_group::2): one pair computes a 256 x 512 tile as two M=256, N=256 MMAs per
-// K step.  Each CTA stages only its own 128 columns of A and its 128-column half of each B tile, so the shared-memory
-// traffic per MMA drops from 12 KB (1-CTA 128 x 256) to 8 KB and the L2 -> SM traffic halves; the 1-CTA kernel
-// saturates shared-memory bandwidth at ~2/3 of the tensor peak (profiles/README.md).
-// =====================================================================================
-// F16 = true: fp16 operands (kind::f16, K = 16 per MMA, 64-element = 128 B boxes, plain 128 B swizzle, 64-row stages);
-// F16 = false: tf32 (fp32 containers, K = 8, 32-element boxes, SWIZZLE_128B_BASE32B, 32-row stages).  Same bytes per stage.
-template <bool F16, int STAGES>
-struct Gram2Cfg {
-  static constexpr int PM = 256, PN = 512;          // pair tile
-  static constexpr int SR = F16 ? 64 : 32;          // rows (K) per stage
-  static constexpr int ES = F16 ? 2 : 4;            // operand element size
-  static constexpr int CW = 128 / ES;               // columns per TMA box (128 B)
-  static constexpr int NBOX = 128 / CW;             // boxes per 128 operand columns
-  static constexpr int KI = F16 ? 16 : 8;           // K per MMA instruction
-  static constexpr int A_BYTES = 128 * SR * ES;     // this CTA's 128 columns of A
-  static constexpr int BH_BYTES = 128 * SR * ES;    // this CTA's half (128 columns) of one N=256 B tile
-  static constexpr int STAGE_BYTES = A_BYTES + 2 * BH_BYTES;
-  static constexpr int BOX_BYTES = SR * 128;
-  static constexpr int KSTEP_BYTES = KI * 128;      // start-address advance per MMA
-  static constexpr int SBO = F16 ? 1024 : 512;      // distance between the K groups inside one MMA
-  static constexpr int STAGING_BYTES = 4 * 4096;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 + 256;
-};
-
-template <bool F16, int STAGES>
-__global__ void __launch_bounds__(kGramThreads, 1)
-gram2_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
-                const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmOut0,
-                const __grid_constant__ CUtensorMap tmOut1, const GramTile* __restrict__ tiles, int num_tiles, int rows,
-                int chunk_rows, int n_valid0, int n_valid1, int epi_multi) {
-  using Cfg = Gram2Cfg<F16, STAGES>;
-  constexpr int SR = Cfg::SR;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();  // 0 = leader (issues the MMAs), 1 = peer
-  const int work = blockIdx.x >> 1;
-  const GramTile tile = tiles[work % num_tiles];
-  const int chunk = work / num_tiles;
-  const int row0 = chunk * chunk_rows;
-  const int nrows = min(chunk_rows, rows - row0);
-  const int ksteps = (nrows + SR - 1) / SR;
-  const int m0 = tile.m_blk * Cfg::PM + static_cast<int>(rank) * 128;  // this CTA's 128 output rows / A columns
-  const int n0 = tile.n_blk * Cfg::PN;
+  const int m0 = tile.m_blk * kTileM;
+  const int n0 = tile.n_blk * kTileN;
   const CUtensorMap* tmB = tile.which ? &tmB1 : &tmB0;
   const CUtensorMap* tmOut = tile.which ? &tmOut1 : &tmOut0;
 
-  if (warp == 0 && elect_one()) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(tmB);
     tma_prefetch_desc(tmOut);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(&full_bar[s], 1);   // leader: its producer's arrive.expect_tx; bytes come from both CTAs
-        mbar_init(&empty_bar[s], 1);  // one multicast commit per use
-      }
-      mbar_init(tmem_full_bar, 1);
-      fence_barrier_init();
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&L.full_bar[s], 1);
+      mbar_init(&L.empty_bar[s], 8);  // one arrive per consumer warp
     }
-    __syncwarp();
-    tmem_alloc_pair(tmem_slot, 512);
-    tmem_relinquish_pair();
+    fence_barrier_init();
   }
-  tc_fence_before();
-  cluster_sync_all();  // both CTAs' barriers are initialised before any remote arrive / complete_tx can land
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (wg == 0) {
+    if (warp == 0 && elect_one()) {
       for (int ks = 0; ks < ksteps; ++ks) {
-        const int s = ks % STAGES;
-        const uint32_t ph = (ks / STAGES) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        if (rank == 0) mbar_arrive_expect_tx(&full_bar[s], 2 * Cfg::STAGE_BYTES);
-        uint8_t* sA = smem + s * Cfg::STAGE_BYTES;
+        const int s = ks % kStages;
+        const uint32_t ph = (ks / kStages) & 1;
+        mbar_wait(&L.empty_bar[s], ph ^ 1);
+        mbar_arrive_expect_tx(&L.full_bar[s], kStageBytes);
+        uint8_t* sA = L.stages + s * kStageBytes;
         uint8_t* sB = sA + Cfg::A_BYTES;
         const int r = row0 + ks * SR;
 #pragma unroll
-        for (int i = 0; i < Cfg::NBOX; ++i) tma_load_2d_pair(sA + i * Cfg::BOX_BYTES, &tmA, &full_bar[s], m0 + Cfg::CW * i, r);
+        for (int i = 0; i < Cfg::NBOX; ++i) tma_load_2d(sA + i * Cfg::BOX_BYTES, &tmA, &L.full_bar[s], m0 + Cfg::CW * i, r);
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int i = 0; i < Cfg::NBOX; ++i)
-            tma_load_2d_pair(sB + h * Cfg::BH_BYTES + i * Cfg::BOX_BYTES, tmB, &full_bar[s],
-                             n0 + h * 256 + static_cast<int>(rank) * 128 + Cfg::CW * i, r);
+        for (int i = 0; i < Cfg::NBOX; ++i) tma_load_2d(sB + i * Cfg::BOX_BYTES, tmB, &L.full_bar[s], n0 + Cfg::CW * i, r);
       }
     }
-  } else if (warp == 1) {
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = F16 ? make_idesc_f16(256, 256, 1, 1) : make_idesc_tf32(256, 256, 1, 1);
-      constexpr uint32_t layout = F16 ? kLayoutSw128 : kLayoutSw128Base32;
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const int s = ks % STAGES;
-        const uint32_t ph = (ks / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t sA = smem_u32(smem + s * Cfg::STAGE_BYTES);
-        const uint32_t sB = sA + Cfg::A_BYTES;
+    return;
+  }
+
+  const int g = wg - 1;  // output rows [64 g, +64) of the tile
+  const int w = warp & 3;
+  float acc[64];
 #pragma unroll
-        for (int kk = 0; kk < SR / Cfg::KI; ++kk) {
-          // MN-major: 128 B-wide MN chunks are BOX_BYTES apart (LBO); K groups inside one MMA are SBO apart
-          const uint64_t ad = make_smem_desc(sA + kk * Cfg::KSTEP_BYTES, Cfg::BOX_BYTES, Cfg::SBO, layout);
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+
+  if (F16) {
+    wgmma_fence_acc(acc);
+    int prev = -1;
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const int s = ks % kStages;
+      mbar_wait(&L.full_bar[s], (ks / kStages) & 1);
+      const uint32_t sA = smem_u32(L.stages + s * kStageBytes) + g * Cfg::BOX_BYTES;  // this warpgroup's 64 columns of A
+      const uint32_t sB = smem_u32(L.stages + s * kStageBytes) + Cfg::A_BYTES;
+      wgmma_fence();
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint64_t bd = make_smem_desc(sB + h * Cfg::BH_BYTES + kk * Cfg::KSTEP_BYTES, Cfg::BOX_BYTES, Cfg::SBO, layout);
-            umma_pair<F16>(tmem_base + h * 256, ad, bd, idesc, (ks | kk) != 0);
-          }
-        }
-        umma_commit_pair(&empty_bar[s]);
+      for (int kk = 0; kk < SR / 16; ++kk) {
+        // 16 rows of K per instruction = two 8-row groups 1024 B apart (SBO); B's two 64-column blocks are a box apart (LBO)
+        const uint64_t ad = make_wgmma_desc(sA + kk * 2048, Cfg::BOX_BYTES, 1024);
+        const uint64_t bd = make_wgmma_desc(sB + kk * 2048, Cfg::BOX_BYTES, 1024);
+        wgmma_f16_n128<1, 1>(acc, ad, bd, 1);
       }
-      umma_commit_pair(tmem_full_bar);
+      wgmma_commit();
+      if (prev >= 0) {
+        wgmma_wait<1>();  // the previous stage's wgmmas have finished reading it
+        if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+      }
+      prev = s;
     }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
   } else {
-    const int q = warp & 3;
-    const int n_valid = tile.which ? n_valid1 : n_valid0;
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    // Once the accumulator is complete nobody reads or writes the operand stages of either CTA any more (every TMA load
-    // has landed and every MMA has retired), so the epilogue rotates through 8 staging buffers per warp carved out of the
-    // stage memory: 8 reduce-adds in flight per warp instead of one store-and-wait round trip per 32-column chunk.
-    uint8_t* buf0 = epi_multi ? smem + (warp - 2) * 32768 : staging + (warp - 2) * 4096;
-    static_assert(STAGES * Cfg::STAGE_BYTES >= 4 * 32768, "stage memory too small for the rotating epilogue buffers");
-#pragma unroll 1
-    for (int c0 = 0; c0 < Cfg::PN; c0 += 32) {
-      if (n0 + c0 >= n_valid) break;  // warp-uniform
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c0, v);
-      tmem_ld_wait();
-      float o[32];
+    // warp tile: rows [32 (w % 2), +32) of the warpgroup's 64, columns [64 (w / 2), +64): 2 x 8 m16n8 fragments
+    const int mrow = 64 * g + 32 * (w & 1);
+    const int ncol = 64 * (w >> 1);
+    const int gq = lane >> 2, tq = lane & 3;
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const int s = ks % kStages;
+      mbar_wait(&L.full_bar[s], (ks / kStages) & 1);
+      const uint8_t* sA = L.stages + s * kStageBytes;
+      const uint8_t* sB = sA + Cfg::A_BYTES;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(v[i]);
-      uint8_t* buf = epi_multi ? buf0 + ((c0 >> 5) & 7) * 4096 : buf0;
-      if (lane == 0) {
-        if (epi_multi) bulk_wait_read7();
-        else bulk_wait_read0();
+      for (int k = 0; k < SR; k += 8) {
+        uint32_t a[2][4], b[8][2];
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi) {
+          const int m = mrow + 16 * mi + gq;
+          a[mi][0] = ld_mn_tf32<Cfg::BOX_BYTES>(sA, m, k + tq);
+          a[mi][1] = ld_mn_tf32<Cfg::BOX_BYTES>(sA, m + 8, k + tq);
+          a[mi][2] = ld_mn_tf32<Cfg::BOX_BYTES>(sA, m, k + tq + 4);
+          a[mi][3] = ld_mn_tf32<Cfg::BOX_BYTES>(sA, m + 8, k + tq + 4);
+        }
+#pragma unroll
+        for (int ni = 0; ni < 8; ++ni) {
+          const int n = ncol + 8 * ni + gq;
+          b[ni][0] = ld_mn_tf32<Cfg::BOX_BYTES>(sB, n, k + tq);
+          b[ni][1] = ld_mn_tf32<Cfg::BOX_BYTES>(sB, n, k + tq + 4);
+        }
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+          for (int ni = 0; ni < 8; ++ni) mma_tf32_16x8x8(&acc[(mi * 8 + ni) * 4], a[mi], b[ni]);
       }
       __syncwarp();
-      stage_row_sw128(buf, lane, o);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        tma_reduce_add_2d(tmOut, buf, n0 + c0, m0 + q * 32);
-        bulk_commit();
-      }
+      if (lane == 0) mbar_arrive(&L.empty_bar[s]);
     }
-    if (lane == 0) bulk_wait0();
-    tc_fence_before();
   }
-  tc_fence_before();
-  cluster_sync_all();  // the peer's shared memory and barriers stay valid until the leader's MMAs / commits are done
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
-  }
+
+  // epilogue: every 32 x 32 chunk of the partial tile is added to the fp32 output with one TMA reduce-add (clipped at the
+  // matrix edge by the map); whole chunks beyond n_valid are skipped
+  const int n_valid = tile.which ? n_valid1 : n_valid0;
+  uint8_t* buf = L.staging + (warp - 4) * 4096;
+  float* raw = L.raw + g * 64 * kRawLd;
+  auto to_raw = [&](float* rw, int slab) {
+    if (F16) {
+      wgmma_acc_to_raw(acc, rw, slab, w, lane);
+    } else if ((w >> 1) == slab) {  // the two warps whose 64 columns are this slab
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < 8; ++ni)
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            rw[(32 * (w & 1) + 16 * mi + (lane >> 2) + 8 * (e >> 1)) * kRawLd + 8 * ni + 2 * (lane & 3) + (e & 1)] =
+                acc[(mi * 8 + ni) * 4 + e];
+    }
+  };
+  auto chunk_fn = [&](float (&o)[32], int, int r_off, int c_off) {
+    const int col = n0 + c_off;
+    if (col >= n_valid) return;  // warp-uniform
+    if (lane == 0) bulk_wait_read0();  // previous chunk's reduce has finished reading the staging buffer
+    __syncwarp();
+    stage_row_sw128(buf, lane, o);
+    fence_proxy_async();
+    __syncwarp();
+    if (lane == 0) {
+      tma_reduce_add_2d(tmOut, buf, col, m0 + 64 * g + r_off);
+      bulk_commit();
+    }
+  };
+  epilogue_slabs(raw, g, w, lane, to_raw, chunk_fn);
+  if (lane == 0) bulk_wait0();
 }
 
 // =====================================================================================
-// K-major GEMM with fused epilogues (persistent, double-buffered TMEM accumulator)
+// K-major GEMM with fused epilogues (persistent)
 // =====================================================================================
-static constexpr int kKmThreads = 576;  // warp 0: TMA, warp 1: MMA + TMEM owner, warps 2-17: epilogue (4 per TMEM lane quarter:
-                                        // the cosine epilogue is issue-bound; with 2 warps per scheduler it ran at IPC ~0.5)
-static constexpr int kKmEpiWarps = 16;
-
-template <bool F16, int BN, int STAGES>
-struct KmCfg {
-  static constexpr int BM = 128;
-  static constexpr int BK = F16 ? 64 : 32;  // K elements per stage: 128 B = one swizzle row
-  static constexpr int ES = F16 ? 2 : 4;
-  static constexpr int A_BYTES = BM * BK * ES;
-  static constexpr int B_BYTES = BN * BK * ES;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGING_BYTES = kKmEpiWarps * 4096;  // one 32 x 32 fp32 chunk per epilogue warp
-  static constexpr int VEC_BYTES = kKmEpiWarps * 128 * 4;   // per-warp bias / shift vectors (64 + 64 columns)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + VEC_BYTES + 1024 + 256;
-};
-
 __device__ __forceinline__ float cos_reduced(float x) {
   // Cody-Waite reduction to [-pi, pi] (round-to-nearest multiple of 2 pi via the 1.5 * 2^23 trick: FMA pipe only),
   // then the SFU cosine (abs err ~ 5e-7 on the reduced range)
@@ -406,466 +329,276 @@ __device__ __forceinline__ void stage_row_f16x2(uint8_t* buf, int lane, const fl
   }
 }
 
-// F16: fp16 operands (kind::f16); OUT16 (EPI_COS only): 1 = the slab is written as fp16 (tmOut: {32, 32} fp16 boxes, no swizzle),
-// 2 = as two fp16 planes hi + lo of the unrounded value (tmOut / tmOut2), the operand pair of the split-operand Gram and update.
-template <int EPI, bool F16, int OUT16, int BN, int STAGES>
-__global__ void __launch_bounds__(kKmThreads, 1)
+// One 32 x 32 chunk of the K-major epilogue: lane holds row row0 + lane, columns col0 + i, as the raw accumulator a[i];
+// vs[0, 32) / vs[32, 64) are vec0 / vec1 of those columns.  slot alternates the two 2 KB halves of the staging buffer for
+// single fp16 outputs, so that one store may still be reading while the next chunk is staged.
+template <int EPI, int OUT16>
+__device__ __forceinline__ void km_chunk(const KmParams& p, const CUtensorMap* tmOut, const CUtensorMap* tmOut2, const float (&a)[32],
+                                         const float* vs, uint8_t* sbuf, int slot, int row0, int col0, int lane, float ascale) {
+  const float* v0s = vs;
+  const float* v1s = vs + 32;
+  float o[32];
+  if (EPI == EPI_COS) {
+    // cosine random feature, or (KM_FLAG_RECT) a rectified linear feature max(floor, z - alpha): PaddedFFT + LinearRectifier.
+    // The value summed into colsum must be exactly the stored one: tf32 rounding here; the fp16 slab is rounded once,
+    // by the packed conversion of the staging step, and its column sums are taken from the staged halfs.
+    if (p.flags & KM_FLAG_RECT) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const float val = fmaxf(p.rect_floor, fmaf(a[i], ascale, -v0s[i])) - v1s[i];
+        o[i] = OUT16 ? val : ((p.flags & KM_FLAG_NO_ROUND) ? val : round_tf32(val));
+      }
+    } else if (p.flags & KM_FLAG_NO_ROUND) {  // unrounded output (parity mode, materialised features): exact range reduction
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[i] = cos_reduced(fmaf(a[i], ascale, v0s[i])) - v1s[i];
+    } else {
+      // 10-bit slabs: cos.approx on the raw argument (its own range reduction costs ~6e-8 |z| of phase: 1e-6 at |z| = 16,
+      // three orders below the operand rounding) saves the four Cody-Waite instructions per element
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const float val = __cosf(fmaf(a[i], ascale, v0s[i])) - v1s[i];
+        o[i] = OUT16 ? val : round_tf32(val);
+      }
+    }
+  } else if (EPI == EPI_UPDATE) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = v0s[i] - a[i] * ascale;
+  } else if (EPI == EPI_APPLY) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = v0s[i] + a[i] * ascale;
+  }
+  if (EPI == EPI_POOL) {
+    // Convolver -> SymmetricRectifier -> sum Pooler: the chunk (32 patch rows x 32 filters) is transposed through the staging
+    // buffer; lane c then owns filter column c and walks the 32 rows, adding max(floor, +-v - alpha) into the pools the row's
+    // patch position belongs to (bit mask per position; rows of a chunk may belong to two images), and flushes the pool
+    // sums of an image with fp32 atomics into out[img][pool * 2 N + {0, N} + filter] (the ImageVectorizer order).
+    uint8_t* buf = sbuf;
+    const int grow = row0 + lane;
+    const int my_img = grow / p.patches_per_image;
+    const unsigned my_mask = grow < p.M ? __ldg(p.pool_mask + (grow - my_img * p.patches_per_image)) : 0u;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = a[i] * ascale;
+    __syncwarp();
+    stage_row_sw128(buf, lane, o);
+    __syncwarp();
+    const int f = col0 + lane;
+    // pool loops are compile-time unrolled over 4 (the CIFAR geometry: 2 x 2 pools) or 16 accumulator pairs
+    auto run = [&](auto np_tag) {
+      constexpr int NP = decltype(np_tag)::value;
+      float ap[NP], an[NP];
+#pragma unroll
+      for (int pl = 0; pl < NP; ++pl) ap[pl] = an[pl] = 0.f;
+      int cur = __shfl_sync(0xffffffffu, my_img, 0);
+      unsigned touched = 0;
+      auto flush = [&](int img) {
+        if (f < p.N && touched) {
+          float* dst = p.pool_out + static_cast<int64_t>(img) * p.pool_out_ld + f;
+#pragma unroll
+          for (int pl = 0; pl < NP; ++pl)
+            if (touched >> pl & 1) {
+              atomicAdd(dst + static_cast<int64_t>(pl) * 2 * p.N, ap[pl]);
+              atomicAdd(dst + static_cast<int64_t>(pl) * 2 * p.N + p.N, an[pl]);
+              ap[pl] = an[pl] = 0.f;
+            }
+        }
+        touched = 0;
+      };
+#pragma unroll 1
+      for (int r = 0; r < 32; ++r) {
+        const int im = __shfl_sync(0xffffffffu, my_img, r);
+        const unsigned mk = __shfl_sync(0xffffffffu, my_mask, r);
+        if (im != cur) {  // warp-uniform
+          flush(cur);
+          cur = im;
+        }
+        if (mk) {
+          const float val = *reinterpret_cast<const float*>(buf + r * 128 + ((((lane >> 2) ^ (r & 7)) << 4) | ((lane & 3) << 2)));
+          const float pos = fmaxf(p.rect_floor, val - p.pool_alpha), neg = fmaxf(p.rect_floor, -val - p.pool_alpha);
+#pragma unroll
+          for (int pl = 0; pl < NP; ++pl)
+            if (mk >> pl & 1) {
+              ap[pl] += pos;
+              an[pl] += neg;
+            }
+          touched |= mk;
+        }
+      }
+      flush(cur);
+    };
+    if (p.n_pools <= 4) run(std::integral_constant<int, 4>{});
+    else run(std::integral_constant<int, 16>{});
+    __syncwarp();
+    return;  // no TMA store for this epilogue
+  }
+  if (EPI == EPI_COS && p.colsum != nullptr && row0 + lane >= p.M) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;  // rows past the end must not pollute the column sums
+  }
+  uint8_t* buf = OUT16 == 1 ? sbuf + slot * 2048 : sbuf;  // an fp16 chunk is 2 KB; the hi + lo pair fills both halves
+  if (lane == 0) {  // the store that last used this staging slot has finished reading it
+    if (OUT16 == 1) bulk_wait_read1();
+    else bulk_wait_read0();
+  }
+  __syncwarp();
+  if (OUT16 == 2) stage_row_f16x2(buf, lane, o);
+  else if (OUT16 == 1) stage_row_f16(buf, lane, o);
+  else stage_row_sw128(buf, lane, o);
+  fence_proxy_async();
+  __syncwarp();
+  if (lane == 0) {
+    if (OUT16 == 2) {
+      tma_store_2d(tmOut, buf, col0, row0);
+      tma_store_2d(tmOut2, buf + 2048, col0, row0);
+    } else if (p.flags & KM_FLAG_REDUCE) {
+      tma_reduce_add_2d(tmOut, buf, col0, row0);
+    } else {
+      tma_store_2d(tmOut, buf, col0, row0);
+    }
+    bulk_commit();
+  }
+  if (EPI == EPI_COS && p.colsum != nullptr) {
+    // column sums of the chunk straight from the staged copy: lane c adds column c over the 32 rows
+    float cs = 0.f;
+    if (OUT16 == 2) {
+#pragma unroll
+      for (int r = 0; r < 32; ++r)
+        cs += __half2float(*reinterpret_cast<const __half*>(buf + r * 64 + lane * 2)) +
+              __half2float(*reinterpret_cast<const __half*>(buf + 2048 + r * 64 + lane * 2));
+    } else if (OUT16 == 1) {
+#pragma unroll
+      for (int r = 0; r < 32; ++r) cs += __half2float(*reinterpret_cast<const __half*>(buf + r * 64 + lane * 2));
+    } else {
+      // (row r keeps 16 B chunk j at (j ^ (r & 7)): 32 lanes read 32 distinct words of one 128 B row, no conflicts)
+#pragma unroll
+      for (int r = 0; r < 32; ++r)
+        cs += *reinterpret_cast<const float*>(buf + r * 128 + ((((lane >> 2) ^ (r & 7)) << 4) | ((lane & 3) << 2)));
+    }
+    const int n = col0 + lane;
+    if (n < p.N) atomicAdd(p.colsum + n, cs);
+  }
+}
+
+// F16: fp16 operands (64 K-elements per 128 B row, K = 16 per wgmma), else tf32 (32 per row, K = 8).  A stage is the
+// 128 x 128 B A tile and the 128 x 128 B B tile, both K-major with 128 B swizzle.  OUT16 (EPI_COS only): 1 = the slab is
+// written as fp16 (tmOut: {32, 32} fp16 boxes, no swizzle), 2 = as two fp16 planes hi + lo of the unrounded value
+// (tmOut / tmOut2), the operand pair of the split-operand Gram and update.
+template <int EPI, bool F16, int OUT16>
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2, KmParams p) {
-  using Cfg = KmCfg<F16, BN, STAGES>;
-  static_assert(BN == 256, "epilogue column split assumes BN == 256");
+  constexpr int BK = F16 ? 64 : 32;  // K elements per stage: 128 B = one swizzle row
+  constexpr int A_BYTES = kTileM * 128;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-  float* vec_smem = reinterpret_cast<float*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES + Cfg::VEC_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;  // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;      // [2]
-  uint64_t* ring_bar = tempty_bar + 2;       // [8] tile-id ring: the producer publishes, MMA issuer and epilogue warps consume
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ring_bar + 8);
-  int* tile_ring = reinterpret_cast<int*>(tmem_slot + 2);  // [8]
+  const SmemLayout L = carve_smem(smem_raw);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int m_tiles = (p.M + Cfg::BM - 1) / Cfg::BM;
-  const int n_tiles = (p.N + BN - 1) / BN;
+  const int wg = warp >> 2;
+  const int m_tiles = (p.M + kTileM - 1) / kTileM;
+  const int n_tiles = (p.N + kTileN - 1) / kTileN;
   const int total_tiles = m_tiles * n_tiles;
-  const int ksteps = (p.K + Cfg::BK - 1) / Cfg::BK;
-  constexpr uint32_t kTmemCols = tmem_cols_for(2 * BN);
+  const int ksteps = (p.K + BK - 1) / BK;
 
-  if (warp == 0 && elect_one()) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmOut);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&empty_bar[s], 1);
-      }
-      for (int a = 0; a < 2; ++a) {
-        mbar_init(&tfull_bar[a], 1);
-        mbar_init(&tempty_bar[a], kKmEpiWarps);  // one arrive per epilogue warp
-      }
-      for (int r = 0; r < 8; ++r) mbar_init(&ring_bar[r], 1);
-      fence_barrier_init();
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&L.full_bar[s], 1);
+      mbar_init(&L.empty_bar[s], 8);  // one arrive per consumer warp
     }
-    __syncwarp();
-    tmem_alloc(tmem_slot, kTmemCols);
-    tmem_relinquish();
+    for (int r = 0; r < 8; ++r) mbar_init(&L.ring_bar[r], 1);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // Tile schedule.  With p.tile_counter the CTAs draw tiles from a global counter: a CTA that got its SM late (this kernel is
   // persistent and shares the GPU with the factor / solve chains' kernels) simply takes fewer tiles instead of stretching the
   // whole launch by its late start.  Without a counter the tiles are strided statically.  Either way the producer publishes
-  // every tile id (then -1) in an 8-slot ring; it never runs more than ~3 tiles ahead of the epilogue, so slots are free.
-  if (warp == 0) {
-    if (elect_one()) {
+  // every tile id (then -1) in an 8-slot ring; the stage ring keeps it within ~kStages tiles of the consumers, so slots are free.
+  if (wg == 0) {
+    if (warp == 0 && elect_one()) {
       uint32_t it = 0, tl = 0;
       int next = p.tile_counter ? atomicAdd(p.tile_counter, 1) : static_cast<int>(blockIdx.x);
       for (;; ++tl) {
         const int t = next < total_tiles ? next : -1;
-        tile_ring[tl & 7] = t;
-        mbar_arrive(&ring_bar[tl & 7]);
+        L.tile_ring[tl & 7] = t;
+        mbar_arrive(&L.ring_bar[tl & 7]);
         if (t < 0) break;
         next = p.tile_counter ? atomicAdd(p.tile_counter, 1) : t + static_cast<int>(gridDim.x);  // latency hides under this tile
-        const int m0 = (t / n_tiles) * Cfg::BM;
-        const int n0 = (t % n_tiles) * BN;
+        const int m0 = (t / n_tiles) * kTileM;
+        const int n0 = (t % n_tiles) * kTileN;
         for (int ks = 0; ks < ksteps; ++ks, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-          uint8_t* sA = smem + s * Cfg::STAGE_BYTES;
-          tma_load_2d(sA, &tmA, &full_bar[s], ks * Cfg::BK, m0);
-          tma_load_2d(sA + Cfg::A_BYTES, &tmB, &full_bar[s], ks * Cfg::BK, n0);
+          const int s = it % kStages;
+          const uint32_t ph = (it / kStages) & 1;
+          mbar_wait(&L.empty_bar[s], ph ^ 1);
+          mbar_arrive_expect_tx(&L.full_bar[s], kStageBytes);
+          uint8_t* sA = L.stages + s * kStageBytes;
+          tma_load_2d(sA, &tmA, &L.full_bar[s], ks * BK, m0);
+          tma_load_2d(sA + A_BYTES, &tmB, &L.full_bar[s], ks * BK, n0);
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = F16 ? make_idesc_f16(Cfg::BM, BN, 0, 0) : make_idesc_tf32(Cfg::BM, BN, 0, 0);
-      uint32_t it = 0, tl = 0;
-      for (;; ++tl) {
-        mbar_wait(&ring_bar[tl & 7], (tl >> 3) & 1);
-        if (tile_ring[tl & 7] < 0) break;
-        const uint32_t a = tl & 1, aph = (tl >> 1) & 1;
-        mbar_wait(&tempty_bar[a], aph ^ 1);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + a * BN;
-        for (int ks = 0; ks < ksteps; ++ks, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sA = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint32_t sB = sA + Cfg::A_BYTES;
+    return;
+  }
+
+  const int g = wg - 1;  // output rows [64 g, +64) of each tile
+  const int w = warp & 3;
+  float* raw = L.raw + g * 64 * kRawLd;
+  float* vs = L.vec + (warp - 4) * 64;
+  uint8_t* sbuf = L.staging + (warp - 4) * 4096;
+  const float ascale = p.acc_scale_ptr ? __ldg(p.acc_scale_ptr) * p.acc_scale : p.acc_scale;
+  uint32_t it = 0;
+  for (uint32_t tl = 0;; ++tl) {
+    mbar_wait(&L.ring_bar[tl & 7], (tl >> 3) & 1);
+    const int t = L.tile_ring[tl & 7];
+    if (t < 0) break;
+    const int m0 = (t / n_tiles) * kTileM;
+    const int n0 = (t % n_tiles) * kTileN;
+
+    float acc[64];
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            // K-major, 128B swizzle: 8-row groups are 1024 B apart (SBO); K advances 32 B (8 tf32 / 16 fp16) per MMA
-            const uint64_t ad = make_smem_desc_sw128(sA + kk * 32, 16, 1024);
-            const uint64_t bd = make_smem_desc_sw128(sB + kk * 32, 16, 1024);
-            if (F16) umma_f16(d_tmem, ad, bd, idesc, (ks | kk) != 0);
-            else umma_tf32(d_tmem, ad, bd, idesc, (ks | kk) != 0);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tfull_bar[a]);
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    wgmma_fence_acc(acc);
+    int prev = -1;
+    for (int ks = 0; ks < ksteps; ++ks, ++it) {
+      const int s = it % kStages;
+      mbar_wait(&L.full_bar[s], (it / kStages) & 1);
+      const uint32_t sA = smem_u32(L.stages + s * kStageBytes) + g * 64 * 128;  // this warpgroup's 64 rows of A
+      const uint32_t sB = smem_u32(L.stages + s * kStageBytes) + A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        // K-major, 128 B swizzle: 8-row groups are 1024 B apart (SBO); K advances 32 B (8 tf32 / 16 fp16) per instruction
+        const uint64_t ad = make_wgmma_desc(sA + kk * 32, 16, 1024);
+        const uint64_t bd = make_wgmma_desc(sB + kk * 32, 16, 1024);
+        if (F16) wgmma_f16_n128<0, 0>(acc, ad, bd, 1);
+        else wgmma_tf32_n128(acc, ad, bd, 1);
       }
+      wgmma_commit();
+      if (prev >= 0) {
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+      }
+      prev = s;
     }
-  } else {
-    // 16 epilogue warps: TMEM lane quarter q = warp % 4 (hardware rule), column quarter (64 columns) = (warp - 2) / 4
-    const int ew = warp - 2;
-    const int q = warp & 3;
-    const int half = ew >> 2;            // column quarter of the 256-wide tile
-    float* v0s = vec_smem + ew * 128;   // this warp's 64 vec0 values
-    float* v1s = v0s + 64;              // and 64 vec1 values
-    uint8_t* buf = staging + ew * 4096;
-    const float ascale = p.acc_scale_ptr ? __ldg(p.acc_scale_ptr) * p.acc_scale : p.acc_scale;
-    uint32_t tl = 0;
-    for (;; ++tl) {
-      mbar_wait(&ring_bar[tl & 7], (tl >> 3) & 1);
-      const int t = tile_ring[tl & 7];
-      if (t < 0) break;
-      const uint32_t a = tl & 1, aph = (tl >> 1) & 1;
-      const int m0 = (t / n_tiles) * Cfg::BM;
-      const int n0 = (t % n_tiles) * BN + half * 64;
-      {  // stage the per-column vectors of this warp's 64 columns in shared memory (broadcast reads below)
-        const int n = n0 + lane * 2;
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          v0s[lane * 2 + j] = (p.vec0 && n + j < p.N) ? __ldg(p.vec0 + n + j) : 0.f;
-          v1s[lane * 2 + j] = (p.vec1 && n + j < p.N) ? __ldg(p.vec1 + n + j) : 0.f;
-        }
-      }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+
+    auto to_raw = [&](float* rw, int slab) { wgmma_acc_to_raw(acc, rw, slab, w, lane); };
+    auto chunk_fn = [&](float (&o)[32], int slab, int r_off, int c_off) {
+      const int col0 = n0 + c_off;
+      if (col0 >= p.N) return;  // warp-uniform
+      __syncwarp();  // the previous chunk's reads of vs are done
+      vs[lane] = (p.vec0 && col0 + lane < p.N) ? __ldg(p.vec0 + col0 + lane) : 0.f;
+      vs[32 + lane] = (p.vec1 && col0 + lane < p.N) ? __ldg(p.vec1 + col0 + lane) : 0.f;
       __syncwarp();
-      mbar_wait(&tfull_bar[a], aph);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        if (n0 + c0 >= p.N) break;  // warp-uniform
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + a * BN + half * 64 + c0, v);
-        tmem_ld_wait();
-        float o[32];
-        if (EPI == EPI_COS) {
-          // cosine random feature, or (KM_FLAG_RECT) a rectified linear feature max(floor, z - alpha): PaddedFFT + LinearRectifier.
-          // The value summed into colsum must be exactly the stored one: tf32 rounding here; the fp16 slab is rounded once,
-          // by the packed conversion of the staging step, and its column sums are taken from the staged halfs.
-          if (p.flags & KM_FLAG_RECT) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float val = fmaxf(p.rect_floor, fmaf(__uint_as_float(v[i]), ascale, -v0s[c0 + i])) - v1s[c0 + i];
-              o[i] = OUT16 ? val : ((p.flags & KM_FLAG_NO_ROUND) ? val : round_tf32(val));
-            }
-          } else if (p.flags & KM_FLAG_NO_ROUND) {  // unrounded output (parity mode, materialised features): exact range reduction
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = cos_reduced(fmaf(__uint_as_float(v[i]), ascale, v0s[c0 + i])) - v1s[c0 + i];
-          } else {
-            // 10-bit slabs: cos.approx on the raw argument (its own range reduction costs ~6e-8 |z| of phase: 1e-6 at |z| = 16,
-            // three orders below the operand rounding) saves the four Cody-Waite instructions per element of this
-            // epilogue-bound kernel (profiles/README.md: 23 warp instructions per 32 elements, tensor pipe 25 % busy)
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float val = __cosf(fmaf(__uint_as_float(v[i]), ascale, v0s[c0 + i])) - v1s[c0 + i];
-              o[i] = OUT16 ? val : round_tf32(val);
-            }
-          }
-        } else if (EPI == EPI_UPDATE) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = v0s[c0 + i] - __uint_as_float(v[i]) * ascale;
-        } else if (EPI == EPI_APPLY) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = v0s[c0 + i] + __uint_as_float(v[i]) * ascale;
-        }
-        if (EPI == EPI_POOL) {
-          // Convolver -> SymmetricRectifier -> sum Pooler: the chunk (32 patch rows x 32 filters) is transposed through the staging
-          // buffer; lane c then owns filter column c and walks the 32 rows, adding max(floor, +-v - alpha) into the pools the row's
-          // patch position belongs to (bit mask per position; rows of a chunk may belong to two images), and flushes the pool
-          // sums of an image with fp32 atomics into out[img][pool * 2 N + {0, N} + filter] (the ImageVectorizer order).
-          const int grow = m0 + q * 32 + lane;
-          const int my_img = grow / p.patches_per_image;
-          const unsigned my_mask = grow < p.M ? __ldg(p.pool_mask + (grow - my_img * p.patches_per_image)) : 0u;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(v[i]) * ascale;
-          __syncwarp();
-          stage_row_sw128(buf, lane, o);
-          __syncwarp();
-          const int f = n0 + c0 + lane;
-          // pool loops are compile-time unrolled over 4 (the CIFAR geometry: 2 x 2 pools) or 16 accumulator pairs
-          auto run = [&](auto np_tag) {
-            constexpr int NP = decltype(np_tag)::value;
-            float ap[NP], an[NP];
-#pragma unroll
-            for (int pl = 0; pl < NP; ++pl) ap[pl] = an[pl] = 0.f;
-            int cur = __shfl_sync(0xffffffffu, my_img, 0);
-            unsigned touched = 0;
-            auto flush = [&](int img) {
-              if (f < p.N && touched) {
-                float* dst = p.pool_out + static_cast<int64_t>(img) * p.pool_out_ld + f;
-#pragma unroll
-                for (int pl = 0; pl < NP; ++pl)
-                  if (touched >> pl & 1) {
-                    atomicAdd(dst + static_cast<int64_t>(pl) * 2 * p.N, ap[pl]);
-                    atomicAdd(dst + static_cast<int64_t>(pl) * 2 * p.N + p.N, an[pl]);
-                    ap[pl] = an[pl] = 0.f;
-                  }
-              }
-              touched = 0;
-            };
-#pragma unroll 1
-            for (int r = 0; r < 32; ++r) {
-              const int im = __shfl_sync(0xffffffffu, my_img, r);
-              const unsigned mk = __shfl_sync(0xffffffffu, my_mask, r);
-              if (im != cur) {  // warp-uniform
-                flush(cur);
-                cur = im;
-              }
-              if (mk) {
-                const float val = *reinterpret_cast<const float*>(buf + r * 128 + ((((lane >> 2) ^ (r & 7)) << 4) | ((lane & 3) << 2)));
-                const float pos = fmaxf(p.rect_floor, val - p.pool_alpha), neg = fmaxf(p.rect_floor, -val - p.pool_alpha);
-#pragma unroll
-                for (int pl = 0; pl < NP; ++pl)
-                  if (mk >> pl & 1) {
-                    ap[pl] += pos;
-                    an[pl] += neg;
-                  }
-                touched |= mk;
-              }
-            }
-            flush(cur);
-          };
-          if (p.n_pools <= 4) run(std::integral_constant<int, 4>{});
-          else run(std::integral_constant<int, 16>{});
-          __syncwarp();
-          continue;  // no TMA store for this epilogue
-        }
-        if (EPI == EPI_COS && p.colsum != nullptr && m0 + q * 32 + lane >= p.M) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = 0.f;  // rows past the end must not pollute the column sums
-        }
-        // an fp16 chunk is 2 KB: the 4 KB staging buffer holds two, so one store may still be reading while the next chunk
-        // is staged (4 chunks per tile: the halves alternate consistently from tile to tile)
-        uint8_t* const sbuf = buf;
-        uint8_t* buf = OUT16 == 1 ? sbuf + ((c0 >> 5) & 1) * 2048 : sbuf;  // the hi + lo pair fills both halves
-        if (lane == 0) {  // the store that last used this staging slot has finished reading it
-          if (OUT16 == 1) bulk_wait_read1();
-          else bulk_wait_read0();
-        }
-        __syncwarp();
-        if (OUT16 == 2) stage_row_f16x2(buf, lane, o);
-        else if (OUT16 == 1) stage_row_f16(buf, lane, o);
-        else stage_row_sw128(buf, lane, o);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          if (OUT16 == 2) {
-            tma_store_2d(&tmOut, buf, n0 + c0, m0 + q * 32);
-            tma_store_2d(&tmOut2, buf + 2048, n0 + c0, m0 + q * 32);
-          } else if (p.flags & KM_FLAG_REDUCE) {
-            tma_reduce_add_2d(&tmOut, buf, n0 + c0, m0 + q * 32);
-          } else {
-            tma_store_2d(&tmOut, buf, n0 + c0, m0 + q * 32);
-          }
-          bulk_commit();
-        }
-        if (EPI == EPI_COS && p.colsum != nullptr) {
-          // column sums of the chunk straight from the staged copy: lane c adds column c over the 32 rows
-          float cs = 0.f;
-          if (OUT16 == 2) {
-#pragma unroll
-            for (int r = 0; r < 32; ++r)
-              cs += __half2float(*reinterpret_cast<const __half*>(buf + r * 64 + lane * 2)) +
-                    __half2float(*reinterpret_cast<const __half*>(buf + 2048 + r * 64 + lane * 2));
-          } else if (OUT16 == 1) {
-#pragma unroll
-            for (int r = 0; r < 32; ++r) cs += __half2float(*reinterpret_cast<const __half*>(buf + r * 64 + lane * 2));
-          } else {
-            // (row r keeps 16 B chunk j at (j ^ (r & 7)): 32 lanes read 32 distinct words of one 128 B row, no conflicts)
-#pragma unroll
-            for (int r = 0; r < 32; ++r)
-              cs += *reinterpret_cast<const float*>(buf + r * 128 + ((((lane >> 2) ^ (r & 7)) << 4) | ((lane & 3) << 2)));
-          }
-          const int n = n0 + c0 + lane;
-          if (n < p.N) atomicAdd(p.colsum + n, cs);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[a]);
-    }
-    if (lane == 0) bulk_wait0();
+      km_chunk<EPI, OUT16>(p, &tmOut, &tmOut2, o, vs, sbuf, slab & 1, m0 + 64 * g + r_off, col0, lane, ascale);
+    };
+    epilogue_slabs(raw, g, w, lane, to_raw, chunk_fn);
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-}
-
-// =====================================================================================
-// K-major GEMM on CTA pairs (cta_group::2) for the two K = blockSize GEMMs (residual update, model apply):
-// one pair computes a 256 x 512 output tile (two M=256, N=256 MMAs per K step); each CTA stages its own 128 rows of A
-// and its 128-row half of each 256-row B tile.  Same shared-memory argument as gram2_tn_kernel: 8 KB instead of 12 KB of
-// operand reads per MMA.  All 512 TMEM columns hold the accumulator, so the epilogue is not overlapped with the next
-// tile's main loop; with K = 4096 it is ~5 % of the tile time.
-// =====================================================================================
-template <bool F16, int STAGES>
-struct Km2Cfg {
-  static constexpr int PM = 256, PN = 512;
-  static constexpr int BK = F16 ? 64 : 32;  // K elements per stage (one 128 B swizzle row)
-  static constexpr int ES = F16 ? 2 : 4;
-  static constexpr int A_BYTES = 128 * BK * ES;
-  static constexpr int BH_BYTES = 128 * BK * ES;
-  static constexpr int STAGE_BYTES = A_BYTES + 2 * BH_BYTES;
-  static constexpr int STAGING_BYTES = 4 * 4096;
-  static constexpr int VEC_BYTES = 4 * 512 * 4;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + VEC_BYTES + 1024 + 256;
-};
-
-template <int EPI, bool F16, int STAGES>
-__global__ void __launch_bounds__(kGramThreads, 1)
-gemm2_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmOut, KmParams p) {
-  using Cfg = Km2Cfg<F16, STAGES>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-  float* vec_smem = reinterpret_cast<float*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES + Cfg::VEC_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int n_tiles = (p.N + Cfg::PN - 1) / Cfg::PN;
-  const int t = blockIdx.x >> 1;
-  const int m0 = (t / n_tiles) * Cfg::PM + static_cast<int>(rank) * 128;
-  const int n0 = (t % n_tiles) * Cfg::PN;
-  const int ksteps = (p.K + Cfg::BK - 1) / Cfg::BK;
-
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmOut);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&empty_bar[s], 1);
-      }
-      mbar_init(tmem_full_bar, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc_pair(tmem_slot, 512);
-    tmem_relinquish_pair();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const int s = ks % STAGES;
-        const uint32_t ph = (ks / STAGES) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        if (rank == 0) mbar_arrive_expect_tx(&full_bar[s], 2 * Cfg::STAGE_BYTES);
-        uint8_t* sA = smem + s * Cfg::STAGE_BYTES;
-        tma_load_2d_pair(sA, &tmA, &full_bar[s], ks * Cfg::BK, m0);
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          tma_load_2d_pair(sA + Cfg::A_BYTES + h * Cfg::BH_BYTES, &tmB, &full_bar[s], ks * Cfg::BK,
-                           n0 + h * 256 + static_cast<int>(rank) * 128);
-      }
-    }
-  } else if (warp == 1) {
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = F16 ? make_idesc_f16(256, 256, 0, 0) : make_idesc_tf32(256, 256, 0, 0);
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const int s = ks % STAGES;
-        const uint32_t ph = (ks / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t sA = smem_u32(smem + s * Cfg::STAGE_BYTES);
-        const uint32_t sB = sA + Cfg::A_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {  // 4 MMAs per 128 B of K (8 tf32 or 16 fp16 elements = 32 B each)
-          const uint64_t ad = make_smem_desc_sw128(sA + kk * 32, 16, 1024);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint64_t bd = make_smem_desc_sw128(sB + h * Cfg::BH_BYTES + kk * 32, 16, 1024);
-            umma_pair<F16>(tmem_base + h * 256, ad, bd, idesc, (ks | kk) != 0);
-          }
-        }
-        umma_commit_pair(&empty_bar[s]);
-      }
-      umma_commit_pair(tmem_full_bar);
-    }
-  } else {
-    const int q = warp & 3;
-    float* v0s = vec_smem + (warp - 2) * 512;
-    const bool epi_multi = (p.flags & KM_FLAG_EPI_MULTI) != 0;  // rotating staging buffers in the idle stage memory (see gram2)
-    uint8_t* buf0 = epi_multi ? smem + (warp - 2) * 32768 : staging + (warp - 2) * 4096;
-    static_assert(STAGES * Cfg::STAGE_BYTES >= 4 * 32768, "stage memory too small for the rotating epilogue buffers");
-    const float ascale = p.acc_scale_ptr ? __ldg(p.acc_scale_ptr) * p.acc_scale : p.acc_scale;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int n = n0 + j * 32 + lane;
-      v0s[j * 32 + lane] = (p.vec0 && n < p.N) ? __ldg(p.vec0 + n) : 0.f;
-    }
-    __syncwarp();
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c0 = 0; c0 < Cfg::PN; c0 += 32) {
-      if (n0 + c0 >= p.N) break;  // warp-uniform
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c0, v);
-      tmem_ld_wait();
-      float o[32];
-      if (EPI == EPI_UPDATE) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = v0s[c0 + i] - __uint_as_float(v[i]) * ascale;
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = v0s[c0 + i] + __uint_as_float(v[i]) * ascale;
-      }
-      uint8_t* buf = epi_multi ? buf0 + ((c0 >> 5) & 7) * 4096 : buf0;
-      if (lane == 0) {
-        if (epi_multi) bulk_wait_read7();
-        else bulk_wait_read0();
-      }
-      __syncwarp();
-      stage_row_sw128(buf, lane, o);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        if (p.flags & KM_FLAG_REDUCE) tma_reduce_add_2d(&tmOut, buf, n0 + c0, m0 + q * 32);
-        else tma_store_2d(&tmOut, buf, n0 + c0, m0 + q * 32);
-        bulk_commit();
-      }
-    }
-    if (lane == 0) bulk_wait0();
-    tc_fence_before();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
-  }
+  if (lane == 0) bulk_wait0();
 }
 
 // =====================================================================================
@@ -889,9 +622,8 @@ static PFN_encodeTiled get_encode_fn() {
 }
 
 // 2D fp32 row-major matrix [rows x cols], leading dimension ld (floats); box = {32 floats, box_rows}, 128B swizzle
-// (atom32: the 32 B-atom flavour required by MN-major tf32 MMA operands).
-int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows, bool atom32) {
-  return make_tmap_any(out, base, rows, cols, ld, 32, box_rows, 4, atom32 ? TMAP_SW128_ATOM32 : TMAP_SW128);
+int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  return make_tmap_any(out, base, rows, cols, ld, 32, box_rows, 4, TMAP_SW128);
 }
 
 // General form: elem_bytes 4 (fp32 / tf32) or 2 (fp16); ld in elements; box {box_cols, box_rows}.
@@ -903,133 +635,70 @@ int make_tmap_any(CUtensorMap* out, const void* base, int64_t rows, int64_t cols
   cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * static_cast<cuuint64_t>(elem_bytes)};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1u, 1u};
-  const CUtensorMapSwizzle sw = swizzle == TMAP_SW128_ATOM32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
-                                : swizzle == TMAP_SW128      ? CU_TENSOR_MAP_SWIZZLE_128B
-                                                             : CU_TENSOR_MAP_SWIZZLE_NONE;
+  const CUtensorMapSwizzle sw = swizzle == TMAP_SW128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE;
   CUresult r = fn(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : -static_cast<int>(r) - 1000;
 }
 
-template <int BN, int SR, int STAGES>
-static cudaError_t launch_gram_t(const GramLaunch& g, cudaStream_t st) {
-  using Cfg = GramCfg<BN, SR, STAGES>;
-  auto kern = gram_tn_kernel<BN, SR, STAGES>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+// The kernels of one family share a signature, so the "attribute set" flag lives in each launcher instantiation.
+template <typename K>
+static cudaError_t set_smem_attr_once(K kern, bool& done) {
+  if (!done) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
     if (e != cudaSuccess) return e;
-    attr_done = true;
+    done = true;
   }
+  return cudaSuccess;
+}
+
+template <bool F16>
+static cudaError_t launch_gram_t(const GramLaunch& g, cudaStream_t st) {
+  if (g.chunk_rows % GramCfg<F16>::SR != 0) return cudaErrorInvalidValue;
+  auto kern = gram_tn_kernel<F16>;
+  static bool attr_done = false;
+  cudaError_t e = set_smem_attr_once(kern, attr_done);
+  if (e != cudaSuccess) return e;
   const int chunks = (g.rows + g.chunk_rows - 1) / g.chunk_rows;
   const unsigned grid = static_cast<unsigned>(chunks) * static_cast<unsigned>(g.num_tiles);
   if (grid == 0) return cudaSuccess;
-  kern<<<grid, kGramThreads, Cfg::SMEM_BYTES, st>>>(g.tmA, g.tmB0, g.tmB1, g.tmOut0, g.tmOut1, g.tiles, g.num_tiles, g.rows,
-                                                   g.chunk_rows, g.n_valid0, g.n_valid1);
+  kern<<<grid, kThreads, kSmemBytes, st>>>(g.tmA, g.tmB0, g.tmB1, g.tmOut0, g.tmOut1, g.tiles, g.num_tiles, g.rows, g.chunk_rows,
+                                           g.n_valid0, g.n_valid1);
   return cudaGetLastError();
-}
-
-template <bool F16, int STAGES>
-static cudaError_t launch_gram2_t(const GramLaunch& g, cudaStream_t st) {
-  using Cfg = Gram2Cfg<F16, STAGES>;
-  if (g.chunk_rows % Cfg::SR != 0) return cudaErrorInvalidValue;
-  auto kern = gram2_tn_kernel<F16, STAGES>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    attr_done = true;
-  }
-  const int chunks = (g.rows + g.chunk_rows - 1) / g.chunk_rows;
-  const unsigned grid = 2u * static_cast<unsigned>(chunks) * static_cast<unsigned>(g.num_tiles);
-  if (grid == 0) return cudaSuccess;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(kGramThreads);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, g.tmA, g.tmB0, g.tmB1, g.tmOut0, g.tmOut1, g.tiles, g.num_tiles, g.rows, g.chunk_rows,
-                            g.n_valid0, g.n_valid1, g.epi_multi);
 }
 
 cudaError_t launch_gram(const GramLaunch& g, cudaStream_t st) {
-  if (g.f16) return launch_gram2_t<true, 4>(g, st);
-  if (g.chunk_rows % kGramStageRows != 0) return cudaErrorInvalidValue;
-  if (g.pair) return launch_gram2_t<false, 4>(g, st);
-  return launch_gram_t<256, kGramStageRows, 4>(g, st);
+  return g.f16 ? launch_gram_t<true>(g, st) : launch_gram_t<false>(g, st);
 }
 
-template <int EPI, bool F16, int OUT16, int BN, int STAGES>
+template <int EPI, bool F16, int OUT16>
 static cudaError_t launch_km_t(const KmLaunch& k, cudaStream_t st) {
-  using Cfg = KmCfg<F16, BN, STAGES>;
-  auto kern = gemm_kmajor_kernel<EPI, F16, OUT16, BN, STAGES>;
+  auto kern = gemm_kmajor_kernel<EPI, F16, OUT16>;
   static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    attr_done = true;
-  }
-  const int m_tiles = (k.p.M + Cfg::BM - 1) / Cfg::BM;
-  const int n_tiles = (k.p.N + BN - 1) / BN;
+  cudaError_t e = set_smem_attr_once(kern, attr_done);
+  if (e != cudaSuccess) return e;
+  const int m_tiles = (k.p.M + kTileM - 1) / kTileM;
+  const int n_tiles = (k.p.N + kTileN - 1) / kTileN;
   const long long total = static_cast<long long>(m_tiles) * n_tiles;
   if (total == 0) return cudaSuccess;
   const unsigned grid = static_cast<unsigned>(total < k.num_sms ? total : k.num_sms);
-  kern<<<grid, kKmThreads, Cfg::SMEM_BYTES, st>>>(k.tmA, k.tmB, k.tmOut, OUT16 == 2 ? k.tmOut2 : k.tmOut, k.p);
+  kern<<<grid, kThreads, kSmemBytes, st>>>(k.tmA, k.tmB, k.tmOut, OUT16 == 2 ? k.tmOut2 : k.tmOut, k.p);
   return cudaGetLastError();
 }
 
-template <int EPI, bool F16, int STAGES>
-static cudaError_t launch_km2_t(const KmLaunch& k, cudaStream_t st) {
-  using Cfg = Km2Cfg<F16, STAGES>;
-  auto kern = gemm2_kmajor_kernel<EPI, F16, STAGES>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    attr_done = true;
-  }
-  const long long m_tiles = (k.p.M + Cfg::PM - 1) / Cfg::PM;
-  const long long n_tiles = (k.p.N + Cfg::PN - 1) / Cfg::PN;
-  const long long total = m_tiles * n_tiles;
-  if (total == 0) return cudaSuccess;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(2 * total));
-  cfg.blockDim = dim3(kGramThreads);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, k.tmA, k.tmB, k.tmOut, k.p);
-}
-
 cudaError_t launch_kmajor(const KmLaunch& k, cudaStream_t st) {
-  if (k.epi == EPI_POOL) return k.f16 ? launch_km_t<EPI_POOL, true, 0, 256, 3>(k, st) : cudaErrorInvalidValue;
-  if (k.epi == EPI_APPLY && k.f16 && !k.pair) return launch_km_t<EPI_APPLY, true, 0, 256, 3>(k, st);  // K-concatenated fp16 operands
-  if (k.f16 && k.epi == EPI_UPDATE) return launch_km2_t<EPI_UPDATE, true, 4>(k, st);
-  if (k.f16 && k.epi == EPI_APPLY) return launch_km2_t<EPI_APPLY, true, 4>(k, st);
-  if (k.out16 == 2 && k.epi == EPI_COS) return k.f16 ? launch_km_t<EPI_COS, true, 2, 256, 3>(k, st) : cudaErrorInvalidValue;
-  if (k.out16 && k.f16 && k.epi == EPI_COS) return launch_km_t<EPI_COS, true, 1, 256, 3>(k, st);
-  if (k.f16 && k.epi == EPI_COS) return launch_km_t<EPI_COS, true, 0, 256, 3>(k, st);  // fp16 operands, fp32 slab (split mode, tf32 pairs)
-  if (k.out16 && k.epi == EPI_COS) return launch_km_t<EPI_COS, false, 1, 256, 3>(k, st);
-  if (k.pair && k.epi == EPI_UPDATE) return launch_km2_t<EPI_UPDATE, false, 4>(k, st);
-  if (k.pair && k.epi == EPI_APPLY) return launch_km2_t<EPI_APPLY, false, 4>(k, st);
+  if (k.epi == EPI_POOL) return k.f16 ? launch_km_t<EPI_POOL, true, 0>(k, st) : cudaErrorInvalidValue;
+  if (k.f16 && k.epi == EPI_APPLY) return launch_km_t<EPI_APPLY, true, 0>(k, st);
+  if (k.f16 && k.epi == EPI_UPDATE) return launch_km_t<EPI_UPDATE, true, 0>(k, st);
+  if (k.out16 == 2 && k.epi == EPI_COS) return k.f16 ? launch_km_t<EPI_COS, true, 2>(k, st) : cudaErrorInvalidValue;
+  if (k.out16 && k.f16 && k.epi == EPI_COS) return launch_km_t<EPI_COS, true, 1>(k, st);
+  if (k.f16 && k.epi == EPI_COS) return launch_km_t<EPI_COS, true, 0>(k, st);  // fp16 operands, fp32 slab (split mode, tf32 pairs)
+  if (k.out16 && k.epi == EPI_COS) return launch_km_t<EPI_COS, false, 1>(k, st);
   switch (k.epi) {
-    case EPI_COS: return launch_km_t<EPI_COS, false, 0, 256, 3>(k, st);
-    case EPI_UPDATE: return launch_km_t<EPI_UPDATE, false, 0, 256, 3>(k, st);
-    case EPI_APPLY: return launch_km_t<EPI_APPLY, false, 0, 256, 3>(k, st);
+    case EPI_COS: return launch_km_t<EPI_COS, false, 0>(k, st);
+    case EPI_UPDATE: return launch_km_t<EPI_UPDATE, false, 0>(k, st);
+    case EPI_APPLY: return launch_km_t<EPI_APPLY, false, 0>(k, st);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -1,5 +1,5 @@
 """Node library of the hot path: same class names, constructor arguments and semantics as the
-reference nodes; the bodies marshal to the C ABI (which launches the sm_100a kernels).
+reference nodes; the bodies marshal to the C ABI (which launches the sm_90a kernels).
 
 Reference classes (K/ = src/main/scala/keystoneml/):
   CosineRandomFeatures                K/nodes/stats/CosineRandomFeatures.scala:19-60

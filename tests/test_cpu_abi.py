@@ -36,14 +36,14 @@ def test_library_exports_every_declared_symbol():
     assert lib.ks_version() >= 100
 
 
-def test_library_has_blackwell_tensor_core_code():
-    """The shipped binary must contain sm_100a tcgen05 / TMA instructions (SASS mnemonics, B200_PROFILING.md)."""
+def test_library_has_hopper_tensor_core_code():
+    """The shipped binary must contain sm_90a wgmma / TMA instructions (SASS mnemonics HGMMA, UTMALDG, UTMASTG)."""
     try:
         sass = subprocess.check_output(["cuobjdump", "-sass", _capi.LIB_PATH], text=True, stderr=subprocess.DEVNULL)
     except (OSError, subprocess.CalledProcessError):
         pytest.skip("cuobjdump not available")
-    assert "UTCHMMA" in sass and "UTMALDG" in sass and "LDTM" in sass
-    assert "sm_100a" in sass
+    assert "HGMMA" in sass and "UTMALDG" in sass and "UTMASTG" in sass
+    assert "sm_90a" in sass
 
 
 def test_no_cpu_fallback():

@@ -23,13 +23,12 @@ def main():
         rfs = [ks.CosineRandomFeatures.create(ctx, d_in, n_out, 0.0555, rng) for _ in range(nrf)]
         feats = ks.Pipeline.gather(rfs).andThen(ks.VectorCombiner())(x)
         est = ks.BlockLeastSquaresEstimator(n_out, 1, 1.0, precision="f16")
-        # (epi_multi, proj_f16, gram_chunk_rows) -- chunk 0 = the engine's own choice
-        configs = [(1, 1, 0), (1, 0, 0), (0, 1, 0), (1, 1, 4096)]
+        # (proj_f16, gram_chunk_rows) -- chunk 0 = the engine's own choice
+        configs = [(1, 0), (0, 0), (1, 4096)]
         if len(sys.argv) > 2:
             configs = [tuple(int(v) for v in c.split(",")) for c in sys.argv[2:]]
         for rep in range(2):
-            for epi, proj, chunk in configs:
-                ctx.set_option("epi_multi", epi)
+            for proj, chunk in configs:
                 ctx.set_option("proj_f16", proj)
                 ctx.set_option("gram_chunk_rows", chunk)
                 est.fit(feats, y)
@@ -39,7 +38,7 @@ def main():
                     est.fit(feats, y)
                     ts.append(1e3 * (time.perf_counter() - t0))
                 st = ctx.last_fit_stats()
-                print(json.dumps({"probe": "ab_fit", "pass": rep, "epi_multi": epi, "proj_f16": proj, "chunk_rows": chunk,
+                print(json.dumps({"probe": "ab_fit", "pass": rep, "proj_f16": proj, "chunk_rows": chunk,
                                   "ms": [round(t, 1) for t in ts], "featurize_ms": st["featurize_ms"], "gram_ms": st["gram_ms"],
                                   "update_ms": st["update_ms"], "solve_ms": st["solve_ms"]}), flush=True)
 
