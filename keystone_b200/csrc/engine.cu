@@ -5,6 +5,7 @@
 // aux_kernels.cu and in cuSOLVER (dense Cholesky of the reduced b x b system); there is no CPU path.
 #include "engine.h"
 
+#include <cuda_fp16.h>
 #include <dlfcn.h>
 #include <stdlib.h>
 #include <math.h>
@@ -607,20 +608,29 @@ const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, i
 
 void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, const void* R, int64_t ldr, int kcols,
                        float* G, int ldg, float* C, int ldc, bool with_g, bool with_c, cudaStream_t st, bool f16,
-                       int64_t chunk_rows) {
+                       int64_t chunk_rows, const void* slab_lo, const void* R_lo) {
   if (rows <= 0 || b <= 0 || (!with_g && !with_c)) return;
   if (!st) st = c.st;
+  const bool split = slab_lo != nullptr;
+  if (split && (!f16 || (with_c && !R_lo))) throw KsError{KS_ERR_INVALID, "split Gram operands must be fp16 pairs"};
   GramLaunch g;
   int nt = 0;
   g.f16 = f16 ? 1 : 0;
+  g.split = split ? 1 : 0;
   g.tiles = gram_tiles(c, b, kcols, with_g, with_c, &nt);
   g.num_tiles = nt;
-  const int stage_rows = f16 ? 64 : kGramStageRows;
-  if (f16) {  // MN-major fp16 operands: 64-column (128 B) x 64-row boxes, plain 128 B swizzle
+  const int stage_rows = split ? 32 : f16 ? 64 : kGramStageRows;
+  if (f16) {  // MN-major fp16 operands: 64-column (128 B) x 64-row boxes (pairs: 32-row), plain 128 B swizzle
     tmap16_or_throw(&g.tmA, slab, rows, b, lds, 64, stage_rows, TMAP_SW128);
     g.tmB0 = g.tmA;
     if (with_c) tmap16_or_throw(&g.tmB1, R, rows, kcols, ldr, 64, stage_rows, TMAP_SW128);
     else g.tmB1 = g.tmA;
+    if (split) {  // the G tiles are A^T A: B0 is A again, lo plane included
+      tmap16_or_throw(&g.tmAlo, slab_lo, rows, b, lds, 64, stage_rows, TMAP_SW128);
+      g.tmB0lo = g.tmAlo;
+      if (with_c) tmap16_or_throw(&g.tmB1lo, R_lo, rows, kcols, ldr, 64, stage_rows, TMAP_SW128);
+      else g.tmB1lo = g.tmAlo;
+    }
   } else {
     tmap_or_throw(&g.tmA, static_cast<const float*>(slab), rows, b, lds, kGramStageRows);
     g.tmB0 = g.tmA;
@@ -647,13 +657,21 @@ void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int 
 
 void launch_update(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, const void* bop, int64_t ldb, int k,
                    float* out, int64_t ldo, const float* cbias, int epi, bool reduce, cudaStream_t st, bool f16,
-                   const float* acc_scale_ptr) {
+                   const float* acc_scale_ptr, const void* slab_lo, const void* bop_lo) {
   if (rows <= 0 || k <= 0 || b <= 0) return;
   if (!st) st = c.st;
+  const bool split = slab_lo != nullptr;
+  if (split && (!f16 || !bop_lo || epi != EPI_UPDATE)) throw KsError{KS_ERR_INVALID, "split update operands must be fp16 pairs"};
   KmLaunch u;
   u.f16 = f16 ? 1 : 0;
+  u.split = split ? 1 : 0;
   u.p.acc_scale_ptr = acc_scale_ptr;
-  if (f16) {  // K-major fp16 operands: 64 K-elements (128 B) x 128 rows per box
+  if (split) {  // four K-major fp16 planes per stage: 32 K-elements (64 B) x 128 rows per box, 64 B swizzle
+    tmap16_or_throw(&u.tmA, slab, rows, b, lds, 32, 128, TMAP_SW64);
+    tmap16_or_throw(&u.tmAlo, slab_lo, rows, b, lds, 32, 128, TMAP_SW64);
+    tmap16_or_throw(&u.tmB, bop, k, b, ldb, 32, 128, TMAP_SW64);
+    tmap16_or_throw(&u.tmBlo, bop_lo, k, b, ldb, 32, 128, TMAP_SW64);
+  } else if (f16) {  // K-major fp16 operands: 64 K-elements (128 B) x 128 rows per box
     tmap16_or_throw(&u.tmA, slab, rows, b, lds, 64, 128, TMAP_SW128);
     tmap16_or_throw(&u.tmB, bop, k, b, ldb, 64, 128, TMAP_SW128);
   } else {
@@ -800,14 +818,18 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   //   features (|value| <= 2: no range problem); the residual and the increments are scaled by device-chosen powers of two.
   //   Materialised feature matrices have arbitrary scale and keep the tf32 path.
   // KS_PRECISION_F16X2 (the parity mode): every MMA operand v is carried as hi + lo (hi = round(v), lo = round(v - hi): 21+
-  //   significant bits) and every product keeps hi*hi + hi*lo + lo*hi, using the same kernels three times (the projection
-  //   once, on operands concatenated along K).  Generated features: fp16 pairs (fp16 MMA); materialised features: tf32
-  //   pairs (tf32 MMA, no range limits).
+  //   significant bits) and every product keeps hi*hi + hi*lo + lo*hi (the projection once, on operands concatenated along
+  //   K).  Generated features: fp16 pairs (fp16 MMA); G, C and the update are each one pass of the split kernels, which load
+  //   the four planes once and reduce-add once.  Materialised features: tf32 pairs (tf32 MMA, no range limits), three passes
+  //   of the single-product kernels, and G keeps the cross Gram S_hi^T S_lo in a second buffer.
   // fp16 slabs only for cosine features (|value| <= 2); rectified linear features have the scale of their input
   const bool x2 = precision == KS_PRECISION_F16X2 && (src.F || src.proj_x2);
   const bool f16 = !src.F && src.kind == 0 && (precision == KS_PRECISION_F16 || x2);
   const size_t es = f16 ? 2 : 4;  // bytes per slab / operand element
   const int64_t x2_chunk = c.split_chunk_rows;  // short accumulation chains: the tensor core's fp32 accumulate truncates
+  // fp16 pairs: every product is one pass of the split kernels (G upper tiles only).  tf32 pairs: three passes, and G keeps the
+  // full S_hi^T S_lo beside its upper S_hi^T S_hi tiles for launch_build_system.
+  const bool g_cross = x2 && !f16;
   // look-ahead of the residual-independent work (projection, G-Gram, factorisation) over the residual chain, in blocks.  With the
   // rows sharded over GPUs the Cholesky of block t+1 (slower next to tensor kernels than alone) sits in a dependency cycle
   // G(t+1) -> factor(t+1) -> solve(t+1) -> update(t+1) -> ... -> G(t+1+LA): a deeper look-ahead spreads it over more blocks.
@@ -845,7 +867,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   const bool cache_factors = num_iter > 1;
   for (int i = 0; i < NBUF; ++i) {
     slab[i].alloc(es * static_cast<size_t>(std::max<int64_t>(n_loc, 1) * lds));
-    gbuf[i].alloc(sizeof(float) * g_elems * (x2 ? 2 : 1));  // x2: S_hi^T S_hi (upper tiles) followed by the full S_hi^T S_lo
+    gbuf[i].alloc(sizeof(float) * g_elems * (g_cross ? 2 : 1));  // S_hi^T S_hi (upper tiles) followed by the full S_hi^T S_lo
     ssum[i].alloc(sizeof(float) * lds);
     if (!cache_factors) Hbuf[i].alloc(sizeof(double) * static_cast<size_t>(bmax) * bmax);
     if (!cache_factors && custom_solve) Dbuf[i].alloc(sizeof(double) * chol_solve_dinv_doubles(bmax));
@@ -975,7 +997,11 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     }
     c.span_begin(PH_GRAM, ST);
     KS_CUDA(cudaMemsetAsync(gbuf[buf].p, 0, gbuf[buf].bytes, ST));
-    if (x2) {  // one launch: upper tiles of S_hi^T S_hi and all tiles of S_hi^T S_lo (the "C" slot with kcols = b)
+    if (x2 && f16) {  // one pass: upper tiles of S_hi^T S_hi + S_lo^T S_hi + S_hi^T S_lo
+      launch_gram_block(c, slab[buf].p, lds, n_loc, b, nullptr, 0, 0, gbuf[buf].as<float>(), ldg, nullptr, 0, true, false, ST, f16,
+                        x2_chunk, slab_lo[buf].p);
+      flops += 4.0 * n_loc * static_cast<double>(b) * b;
+    } else if (x2) {  // one launch: upper tiles of S_hi^T S_hi and all tiles of S_hi^T S_lo (the "C" slot with kcols = b)
       launch_gram_block(c, slab[buf].p, lds, n_loc, b, slab_lo[buf].p, lds, b, gbuf[buf].as<float>(), ldg,
                         gbuf[buf].as<float>() + g_elems, ldg, true, true, ST, f16, x2_chunk);
       flops += 4.0 * n_loc * static_cast<double>(b) * b;
@@ -988,7 +1014,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     if (c.world > 1) {
       if (SG != ST) KS_CUDA(cudaStreamWaitEvent(SG, ev_gdone[t], 0));
       c.span_begin(PH_ALLREDUCE, SG);
-      c.allreduce_on(gbuf[buf].p, g_elems * (x2 ? 2 : 1), false, commG, SG);
+      c.allreduce_on(gbuf[buf].p, g_elems * (g_cross ? 2 : 1), false, commG, SG);
       c.allreduce_on(ssum[buf].p, static_cast<size_t>(b), false, commG, SG);
       if (x2) c.allreduce_on(dsq[buf].p, static_cast<size_t>(b), true, commG, SG);
       c.span_end(SG);
@@ -1018,7 +1044,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     c.span_begin(PH_SOLVE, SF);
     launch_delta_mean(ssum[buf].as<float>(), shifts[j]->as<float>(), n_total_d, deltas[j]->as<double>(), model->mean[j]->as<double>(), b, SF);
     launch_build_system(gbuf[buf].as<float>(), ldg, deltas[j]->as<double>(), n_total_d, lam, Hj, b, SF,
-                        x2 ? gbuf[buf].as<float>() + g_elems : nullptr, x2 ? dsq[buf].as<double>() : nullptr);
+                        g_cross ? gbuf[buf].as<float>() + g_elems : nullptr, x2 ? dsq[buf].as<double>() : nullptr);
     c.launches += 2;
     c.potrf(Hj, b, info_slot++, SF);
     if (Dj) {  // inverses of the factor's 64 x 64 diagonal tiles: the in-tile substitutions of the solve become DMMA products
@@ -1045,9 +1071,15 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     c.span_end(SR);
     if (SR != ST) KS_CUDA(cudaStreamWaitEvent(SR, ev_slab[t], 0));
     c.span_begin(PH_UPDATE, SR);  // A^T R part of the Gram (accounted with the residual chain)
-    launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
-                      x2 ? x2_chunk : 0);
-    if (x2) {  // + S_lo^T R_hi + S_hi^T R_lo, reduce-added into the same C
+    if (x2 && f16) {  // one pass: S_hi^T R_hi + S_lo^T R_hi + S_hi^T R_lo
+      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
+                        x2_chunk, slab_lo[buf].p, r_lo.p);
+      flops += 4.0 * n_loc * static_cast<double>(b) * k;
+    } else {
+      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
+                        x2 ? x2_chunk : 0);
+    }
+    if (x2 && !f16) {  // + S_lo^T R_hi + S_hi^T R_lo, reduce-added into the same C
       launch_gram_block(c, slab_lo[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
                         x2_chunk);
       launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_lo.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
@@ -1128,9 +1160,15 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     const int b = block_cols(j, &c0);
     if (SR != SS) KS_CUDA(cudaStreamWaitEvent(SR, ev_solved[t], 0));
     c.span_begin(PH_UPDATE, SR);
-    launch_update(c, slab[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, cbias.as<float>(),
-                  EPI_UPDATE, /*reduce=*/true, SR, f16, f16 ? dwscale + 1 : nullptr);
-    if (x2) {  // - S_lo dW_hi - S_hi dW_lo (the constant delta^T dW is applied once, above)
+    if (x2 && f16) {  // one pass: R -= S_hi dW_hi + S_lo dW_hi + S_hi dW_lo
+      launch_update(c, slab[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, cbias.as<float>(), EPI_UPDATE,
+                    /*reduce=*/true, SR, f16, dwscale + 1, slab_lo[buf].p, bop_lo.p);
+      flops += 4.0 * n_loc * static_cast<double>(b) * k;
+    } else {
+      launch_update(c, slab[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, cbias.as<float>(),
+                    EPI_UPDATE, /*reduce=*/true, SR, f16, f16 ? dwscale + 1 : nullptr);
+    }
+    if (x2 && !f16) {  // - S_lo dW_hi - S_hi dW_lo (the constant delta^T dW is applied once, above)
       launch_update(c, slab_lo[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, nullptr, EPI_UPDATE, true, SR, f16,
                     f16 ? dwscale + 1 : nullptr);
       launch_update(c, slab[buf].p, lds, n_loc, b, bop_lo.p, lds, k, r_f32.as<float>(), kpad, nullptr, EPI_UPDATE, true, SR, f16,
@@ -2247,19 +2285,55 @@ KS_API int32_t ks_last_fit_stats_json(int64_t ctx, char* buf, int64_t buflen) {
 }
 
 // ---------------------------------------------------------------- debug / micro-benchmarks
-// With the context option precision = KS_PRECISION_F16 the operands are first converted to fp16 and the fp16 kernel runs.
+// With the context option precision = KS_PRECISION_F16 the operands are first converted to fp16 and the fp16 kernel runs;
+// with KS_PRECISION_F16X2 they are split into fp16 pairs hi + lo and the split kernel runs (G = A^T A keeps
+// hi^T hi + lo^T hi + hi^T lo); with KS_PRECISION_TF32 the fp32 operands go to the tf32 kernel as they are.
 struct DebugGramOps {
-  DevBuf a16, b16;
+  DevBuf a16, b16, a16lo, b16lo;
   const void* A = nullptr;
   const void* B = nullptr;
+  const void* Alo = nullptr;
+  const void* Blo = nullptr;
   bool f16 = false;
 };
+__global__ void split_f16_pair_kernel(const float* __restrict__ src, int64_t ld, int64_t rows, int cols, __half* __restrict__ hi,
+                                      __half* __restrict__ lo) {
+  const int64_t total = rows * cols;
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t r = i / cols, o = r * ld + (i - r * cols);
+    const float v = src[o];
+    const __half h = __float2half_rn(v);
+    hi[o] = h;
+    lo[o] = __float2half_rn(v - __half2float(h));
+  }
+}
+static void debug_split_f16(Ctx& c, Matrix& M, DevBuf& hi, DevBuf& lo) {
+  const size_t bytes = 2 * static_cast<size_t>(std::max<int64_t>(M.rows, 1) * M.ld);
+  hi.alloc(bytes);
+  lo.alloc(bytes);
+  KS_CUDA(cudaMemsetAsync(hi.p, 0, bytes, c.st));  // pad columns stay zero
+  KS_CUDA(cudaMemsetAsync(lo.p, 0, bytes, c.st));
+  const int64_t total = M.rows * M.cols;
+  if (total > 0) {
+    const unsigned grid = static_cast<unsigned>(std::min<int64_t>((total + 255) / 256, 4096));
+    split_f16_pair_kernel<<<grid, 256, 0, c.st>>>(M.d, M.ld, M.rows, static_cast<int>(M.cols), hi.as<__half>(), lo.as<__half>());
+    c.launches += 1;
+  }
+}
 static void debug_gram_run(Ctx& c, Matrix& A, Matrix& B, DevBuf& gc, int* ldg, int* ldc, DebugGramOps& ops) {
   if (A.rows != B.rows) throw KsError{KS_ERR_INVALID, "row mismatch"};
-  ops.f16 = c.precision == KS_PRECISION_F16;
+  ops.f16 = c.precision == KS_PRECISION_F16 || c.precision == KS_PRECISION_F16X2;
   ops.A = A.d;
   ops.B = B.d;
-  if (ops.f16) {
+  if (c.precision == KS_PRECISION_F16X2) {
+    debug_split_f16(c, A, ops.a16, ops.a16lo);
+    debug_split_f16(c, B, ops.b16, ops.b16lo);
+    ops.A = ops.a16.p;
+    ops.B = ops.b16.p;
+    ops.Alo = ops.a16lo.p;
+    ops.Blo = ops.b16lo.p;
+  } else if (ops.f16) {
     ops.a16.alloc(2 * static_cast<size_t>(std::max<int64_t>(A.rows, 1) * A.ld));
     ops.b16.alloc(2 * static_cast<size_t>(std::max<int64_t>(B.rows, 1) * B.ld));
     launch_f32_to_f16_rows(A.d, A.ld, ops.a16.p, A.ld, A.rows, A.cols, c.st);
@@ -2274,7 +2348,7 @@ static void debug_gram_run(Ctx& c, Matrix& A, Matrix& B, DevBuf& gc, int* ldg, i
   gc.alloc(sizeof(float) * (ge + ce));
   KS_CUDA(cudaMemsetAsync(gc.p, 0, gc.bytes, c.st));
   launch_gram_block(c, ops.A, A.ld, A.rows, b, ops.B, B.ld, kc, gc.as<float>(), *ldg, gc.as<float>() + ge, *ldc, true, true,
-                    nullptr, ops.f16);
+                    nullptr, ops.f16, 0, ops.Alo, ops.Blo);
 }
 KS_API int32_t ks_debug_gram(int64_t ctx, int64_t a, int64_t b, double* out_g, int64_t ld_g, double* out_c, int64_t ld_c) {
   return guard(ctx, [&](Ctx& c) {
@@ -2311,7 +2385,7 @@ KS_API int32_t ks_debug_time_gram(int64_t ctx, int64_t a, int64_t b, int32_t ite
     KS_CUDA(cudaEventRecord(e0, c.st));
     for (int i = 0; i < iters; ++i)
       launch_gram_block(c, ops.A, A.ld, A.rows, static_cast<int>(A.cols), ops.B, B.ld, static_cast<int>(B.cols), gc.as<float>(),
-                        ldg, gc.as<float>() + ge, ldc, true, true, nullptr, ops.f16);
+                        ldg, gc.as<float>() + ge, ldc, true, true, nullptr, ops.f16, 0, ops.Alo, ops.Blo);
     KS_CUDA(cudaEventRecord(e1, c.st));
     c.check_async("debug_time_gram");
     float ms = 0;

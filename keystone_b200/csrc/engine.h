@@ -281,12 +281,14 @@ const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, i
 // f16: slab and R are fp16 matrices (leading dimensions in elements); G / C stay fp32
 void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, const void* R, int64_t ldr, int kcols,
                        float* G, int ldg, float* C, int ldc, bool with_g, bool with_c, cudaStream_t st = nullptr,
-                       bool f16 = false, int64_t chunk_rows = 0);  // chunk_rows 0: the context's choice
+                       bool f16 = false, int64_t chunk_rows = 0,  // chunk_rows 0: the context's choice
+                       const void* slab_lo = nullptr, const void* R_lo = nullptr);  // fp16 pairs: hi^T hi + lo^T hi + hi^T lo, one pass
 // out[rows x k] (+)= (epi == EPI_UPDATE ? -1 : +1) * slab[rows x b] * bop[k x b]^T + cbias   (reduce: add into out)
 // f16: slab and bop are fp16; the product is multiplied by *acc_scale_ptr (device scalar, may be null) before the epilogue
 void launch_update(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, const void* bop, int64_t ldb, int k,
                    float* out, int64_t ldo, const float* cbias, int epi, bool reduce, cudaStream_t st = nullptr,
-                   bool f16 = false, const float* acc_scale_ptr = nullptr);
+                   bool f16 = false, const float* acc_scale_ptr = nullptr,
+                   const void* slab_lo = nullptr, const void* bop_lo = nullptr);  // fp16 pairs: all three products in one pass
 
 int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double lam, double w, int64_t nf_opt,
                  int precision = KS_PRECISION_TF32);

@@ -18,14 +18,16 @@ struct GramTile {
   int pad;
 };
 struct GramLaunch {
-  CUtensorMap tmA, tmB0, tmB1;   // operands: tf32 box {32, kGramStageRows}, fp16 box {64, 64}; SWIZZLE_128B
+  CUtensorMap tmA, tmB0, tmB1;   // operands: tf32 box {32, kGramStageRows}, fp16 box {64, 64} (split: {64, 32}); SWIZZLE_128B
   CUtensorMap tmOut0, tmOut1;    // outputs:  box {32, 32}, SWIZZLE_128B; dims clip the reduce-add at the matrix edge
+  CUtensorMap tmAlo, tmB0lo, tmB1lo;  // split only: the lo planes of A, B0, B1 (same geometry as the hi maps)
   const GramTile* tiles;         // device
   int num_tiles;
   int rows;        // contraction length (rows of A and B)
-  int chunk_rows;  // split of the contraction across CTAs (multiple of kGramStageRows)
+  int chunk_rows;  // split of the contraction across CTAs (multiple of the stage rows)
   int n_valid0, n_valid1;  // valid output columns per target (whole 32-column chunks beyond are skipped)
   int f16 = 0;             // 1: operands are fp16 (wgmma, 64-row stages), 0: tf32 (mma.sync, 32-row stages)
+  int split = 0;           // 1 (f16 only): operands are fp16 pairs hi + lo, one pass computes hi^T hi + lo^T hi + hi^T lo
 };
 enum { KM_FLAG_NO_ROUND = 1, KM_FLAG_REDUCE = 2, KM_FLAG_RECT = 8 };
 struct KmParams {
@@ -50,16 +52,18 @@ struct KmLaunch {
   CUtensorMap tmA, tmB;  // operands: box {32, 128} (tf32) / {64, 128} (fp16), SWIZZLE_128B
   CUtensorMap tmOut;     // output: box {32, 32}, SWIZZLE_128B
   CUtensorMap tmOut2;    // out16 == 2 only: the lo plane (same geometry as tmOut)
+  CUtensorMap tmAlo, tmBlo;  // split only: lo planes of A and B; then every operand map has box {32, 128}, SWIZZLE_64B
   KmParams p;
   int epi;
   int num_sms;
   int f16 = 0;   // 1: fp16 operands
+  int split = 0; // 1 (EPI_UPDATE, f16 only): operands are fp16 pairs, one pass computes A_hi B_hi^T + A_lo B_hi^T + A_hi B_lo^T
   int out16 = 0; // EPI_COS: 1 = the slab is written as fp16 (tmOut: {32, 32} fp16 boxes, no swizzle); 2 = as the fp16 pair hi + lo
                  // of the unrounded value (tmOut, tmOut2)
 };
 
 int make_tmap_2d(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows);
-enum { TMAP_SW128 = 0, TMAP_NONE = 2 };
+enum { TMAP_SW128 = 0, TMAP_SW64 = 1, TMAP_NONE = 2 };
 int make_tmap_any(CUtensorMap* out, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows,
                   int elem_bytes, int swizzle);
 cudaError_t launch_gram(const GramLaunch& g, cudaStream_t st);

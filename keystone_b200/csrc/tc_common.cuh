@@ -124,15 +124,24 @@ __device__ __forceinline__ void stage_row_sw128(uint8_t* buf, int lane, const fl
 //   [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4
 //   [32,46) stride-dim byte offset >> 4   [49,52) base offset (0: tiles are 1024 B aligned)   [62,64) swizzle: 1 = 128 B
 // K-major 128 B swizzle: rows of 128 B, 8-row groups SBO apart (LBO unused).  MN-major 128 B swizzle: 64 fp16 MN elements per
-// 128 B row, one K index per row; 64-wide MN blocks are LBO apart, 8-row K groups SBO apart.
+// 128 B row, one K index per row; 64-wide MN blocks are LBO apart, 8-row K groups SBO apart.  SW = 2 selects the 64 B swizzle
+// (K-major rows of 64 B, 8-row groups of 512 B; tiles 512 B aligned).
+template <int SW = 1>
 __device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 62;
+  d |= static_cast<uint64_t>(SW) << 62;
   return d;
 }
+
+// Register reallocation between the warpgroups of a CTA (executed by every thread of a warpgroup): the TMA producer gives its
+// registers back, the MMA warpgroups take them, so that two 64-register accumulators per thread fit without spilling.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N) : "memory"); }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

@@ -18,6 +18,8 @@
 // epilogue math -> 128 B-swizzled staging -> TMA store / TMA reduce-add, so global memory only sees full 128 B rows.
 // wgmma accepts tf32 operands only K-major, so the tf32 Gram (MN-major) builds warp-level mma.sync fragments from the same
 // TMA-filled stages instead.
+// SPLIT variants (parity mode, fp16 pairs; Gram and EPI_UPDATE): each stage holds the hi and lo planes of both operands and one
+// pass issues hi·hi, lo·hi and hi·lo into two accumulators, so the operands are fetched and the output is reduce-added once.
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -97,14 +99,17 @@ __device__ __forceinline__ void epilogue_slabs(float* raw, int g, int w, int lan
 // F16: fp16 operands, 64-column (128 B) x 64-row TMA boxes, wgmma with both operands MN-major (K = 16 per instruction);
 // tf32: fp32 containers, 32-column x 32-row boxes, mma.sync m16n8k8 fragments (K = 8).  Either way a stage holds the 128
 // columns of A and of B for SR rows of the contraction: 32 KB.
-template <bool F16>
+// SPLIT (fp16 pairs): a stage holds the four tiles A_hi, A_lo, B_hi, B_lo of 32 rows each (64 x 32 boxes), still 32 KB.
+template <bool F16, bool SPLIT = false>
 struct GramCfg {
-  static constexpr int SR = F16 ? 64 : 32;       // rows (K) per stage
+  static constexpr int PLANES = SPLIT ? 4 : 2;   // operand tiles per stage
+  static constexpr int SR = SPLIT ? 32 : F16 ? 64 : 32;  // rows (K) per stage
   static constexpr int CW = F16 ? 64 : 32;       // columns per TMA box (128 B)
   static constexpr int NBOX = kTileM / CW;       // boxes per 128 operand columns
   static constexpr int BOX_BYTES = SR * 128;
   static constexpr int A_BYTES = NBOX * BOX_BYTES;
-  static_assert(2 * A_BYTES == kStageBytes, "stage size");
+  static_assert(PLANES * A_BYTES == kStageBytes, "stage size");
+  static_assert(!SPLIT || F16, "split operands are fp16 pairs");
 };
 
 // tf32 element (column c, row r) of one MN-major operand tile: 32-column boxes of SR rows, 128 B swizzle
@@ -114,13 +119,17 @@ __device__ __forceinline__ uint32_t ld_mn_tf32(const uint8_t* tile, int c, int r
                                             ((c & 3) << 2));
 }
 
-template <bool F16>
+// SPLIT: D += A_hi^T B_hi + A_lo^T B_hi + A_hi^T B_lo in one pass.  The hi x hi product accumulates in its own registers
+// with the same instruction sequence as the single-product kernel; the two cross products (~2^-11 smaller) share a second
+// accumulator; the two are added (fp32, round-to-nearest) before the epilogue, so each chunk is reduce-added once.
+template <bool F16, bool SPLIT>
 __global__ void __launch_bounds__(kThreads, 1)
 gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
                const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmOut0,
-               const __grid_constant__ CUtensorMap tmOut1, const GramTile* __restrict__ tiles, int num_tiles, int rows,
-               int chunk_rows, int n_valid0, int n_valid1) {
-  using Cfg = GramCfg<F16>;
+               const __grid_constant__ CUtensorMap tmOut1, const __grid_constant__ CUtensorMap tmAlo,
+               const __grid_constant__ CUtensorMap tmB0lo, const __grid_constant__ CUtensorMap tmB1lo,
+               const GramTile* __restrict__ tiles, int num_tiles, int rows, int chunk_rows, int n_valid0, int n_valid1) {
+  using Cfg = GramCfg<F16, SPLIT>;
   constexpr int SR = Cfg::SR;
   extern __shared__ uint8_t smem_raw[];
   const SmemLayout L = carve_smem(smem_raw);
@@ -136,11 +145,16 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int m0 = tile.m_blk * kTileM;
   const int n0 = tile.n_blk * kTileN;
   const CUtensorMap* tmB = tile.which ? &tmB1 : &tmB0;
+  const CUtensorMap* tmBlo = tile.which ? &tmB1lo : &tmB0lo;
   const CUtensorMap* tmOut = tile.which ? &tmOut1 : &tmOut0;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(tmB);
+    if (SPLIT) {
+      tma_prefetch_desc(&tmAlo);
+      tma_prefetch_desc(tmBlo);
+    }
     tma_prefetch_desc(tmOut);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&L.full_bar[s], 1);
@@ -151,6 +165,7 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   __syncthreads();
 
   if (wg == 0) {
+    if (SPLIT) setmaxnreg_dec<40>();  // two accumulators per consumer thread
     if (warp == 0 && elect_one()) {
       for (int ks = 0; ks < ksteps; ++ks) {
         const int s = ks % kStages;
@@ -158,16 +173,21 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         mbar_wait(&L.empty_bar[s], ph ^ 1);
         mbar_arrive_expect_tx(&L.full_bar[s], kStageBytes);
         uint8_t* sA = L.stages + s * kStageBytes;
-        uint8_t* sB = sA + Cfg::A_BYTES;
         const int r = row0 + ks * SR;
+        // tiles in stage order: A, B (SPLIT: A_hi, A_lo, B_hi, B_lo)
+        const CUtensorMap* maps[4] = {&tmA, SPLIT ? &tmAlo : tmB, tmB, tmBlo};
 #pragma unroll
-        for (int i = 0; i < Cfg::NBOX; ++i) tma_load_2d(sA + i * Cfg::BOX_BYTES, &tmA, &L.full_bar[s], m0 + Cfg::CW * i, r);
+        for (int pl = 0; pl < Cfg::PLANES; ++pl) {
+          const int c0 = (pl < Cfg::PLANES / 2) ? m0 : n0;
 #pragma unroll
-        for (int i = 0; i < Cfg::NBOX; ++i) tma_load_2d(sB + i * Cfg::BOX_BYTES, tmB, &L.full_bar[s], n0 + Cfg::CW * i, r);
+          for (int i = 0; i < Cfg::NBOX; ++i)
+            tma_load_2d(sA + pl * Cfg::A_BYTES + i * Cfg::BOX_BYTES, maps[pl], &L.full_bar[s], c0 + Cfg::CW * i, r);
+        }
       }
     }
     return;
   }
+  if (SPLIT) setmaxnreg_inc<232>();
 
   const int g = wg - 1;  // output rows [64 g, +64) of the tile
   const int w = warp & 3;
@@ -175,7 +195,44 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 
-  if (F16) {
+  if (SPLIT) {
+    float acc_x[64];  // lo^T hi + hi^T lo
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc_x[i] = 0.f;
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(acc_x);
+    int prev = -1;
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const int s = ks % kStages;
+      mbar_wait(&L.full_bar[s], (ks / kStages) & 1);
+      const uint32_t st = smem_u32(L.stages + s * kStageBytes);
+      const uint32_t sAhi = st + g * Cfg::BOX_BYTES, sAlo = sAhi + Cfg::A_BYTES;  // this warpgroup's 64 columns of A
+      const uint32_t sBhi = st + 2 * Cfg::A_BYTES, sBlo = st + 3 * Cfg::A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < SR / 16; ++kk)
+        wgmma_f16_n128<1, 1>(acc, make_wgmma_desc(sAhi + kk * 2048, Cfg::BOX_BYTES, 1024),
+                             make_wgmma_desc(sBhi + kk * 2048, Cfg::BOX_BYTES, 1024), 1);
+#pragma unroll
+      for (int kk = 0; kk < SR / 16; ++kk) {
+        wgmma_f16_n128<1, 1>(acc_x, make_wgmma_desc(sAlo + kk * 2048, Cfg::BOX_BYTES, 1024),
+                             make_wgmma_desc(sBhi + kk * 2048, Cfg::BOX_BYTES, 1024), 1);
+        wgmma_f16_n128<1, 1>(acc_x, make_wgmma_desc(sAhi + kk * 2048, Cfg::BOX_BYTES, 1024),
+                             make_wgmma_desc(sBlo + kk * 2048, Cfg::BOX_BYTES, 1024), 1);
+      }
+      wgmma_commit();
+      if (prev >= 0) {
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+      }
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(acc_x);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = __fadd_rn(acc[i], acc_x[i]);
+  } else if (F16) {
     wgmma_fence_acc(acc);
     int prev = -1;
     for (int ks = 0; ks < ksteps; ++ks) {
@@ -482,12 +539,18 @@ __device__ __forceinline__ void km_chunk(const KmParams& p, const CUtensorMap* t
 // 128 x 128 B A tile and the 128 x 128 B B tile, both K-major with 128 B swizzle.  OUT16 (EPI_COS only): 1 = the slab is
 // written as fp16 (tmOut: {32, 32} fp16 boxes, no swizzle), 2 = as two fp16 planes hi + lo of the unrounded value
 // (tmOut / tmOut2), the operand pair of the split-operand Gram and update.
-template <int EPI, bool F16, int OUT16>
+// SPLIT (fp16 pairs): a stage holds A_hi, A_lo, B_hi, B_lo with 32 K-elements each (64 B rows, 64 B swizzle, 8 KB per tile);
+// A_hi B_hi^T accumulates on its own, A_lo B_hi^T + A_hi B_lo^T in a second accumulator, and their fp32 sum goes through the
+// epilogue once.
+template <int EPI, bool F16, int OUT16, bool SPLIT>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2, KmParams p) {
-  constexpr int BK = F16 ? 64 : 32;  // K elements per stage: 128 B = one swizzle row
-  constexpr int A_BYTES = kTileM * 128;
+                   const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2,
+                   const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, KmParams p) {
+  static_assert(!SPLIT || F16, "split operands are fp16 pairs");
+  constexpr int ROW_BYTES = SPLIT ? 64 : 128;     // one swizzle row of K
+  constexpr int BK = ROW_BYTES / (F16 ? 2 : 4);   // K elements per stage
+  constexpr int A_BYTES = kTileM * ROW_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const SmemLayout L = carve_smem(smem_raw);
 
@@ -502,6 +565,10 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (SPLIT) {
+      tma_prefetch_desc(&tmAlo);
+      tma_prefetch_desc(&tmBlo);
+    }
     tma_prefetch_desc(&tmOut);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&L.full_bar[s], 1);
@@ -534,8 +601,15 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           mbar_wait(&L.empty_bar[s], ph ^ 1);
           mbar_arrive_expect_tx(&L.full_bar[s], kStageBytes);
           uint8_t* sA = L.stages + s * kStageBytes;
-          tma_load_2d(sA, &tmA, &L.full_bar[s], ks * BK, m0);
-          tma_load_2d(sA + A_BYTES, &tmB, &L.full_bar[s], ks * BK, n0);
+          if (SPLIT) {  // A_hi, A_lo, B_hi, B_lo
+            tma_load_2d(sA, &tmA, &L.full_bar[s], ks * BK, m0);
+            tma_load_2d(sA + A_BYTES, &tmAlo, &L.full_bar[s], ks * BK, m0);
+            tma_load_2d(sA + 2 * A_BYTES, &tmB, &L.full_bar[s], ks * BK, n0);
+            tma_load_2d(sA + 3 * A_BYTES, &tmBlo, &L.full_bar[s], ks * BK, n0);
+          } else {
+            tma_load_2d(sA, &tmA, &L.full_bar[s], ks * BK, m0);
+            tma_load_2d(sA + A_BYTES, &tmB, &L.full_bar[s], ks * BK, n0);
+          }
         }
       }
     }
@@ -559,32 +633,70 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     float acc[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    wgmma_fence_acc(acc);
-    int prev = -1;
-    for (int ks = 0; ks < ksteps; ++ks, ++it) {
-      const int s = it % kStages;
-      mbar_wait(&L.full_bar[s], (it / kStages) & 1);
-      const uint32_t sA = smem_u32(L.stages + s * kStageBytes) + g * 64 * 128;  // this warpgroup's 64 rows of A
-      const uint32_t sB = smem_u32(L.stages + s * kStageBytes) + A_BYTES;
-      wgmma_fence();
+    if (SPLIT) {
+      float acc_x[64];  // A_lo B_hi^T + A_hi B_lo^T
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        // K-major, 128 B swizzle: 8-row groups are 1024 B apart (SBO); K advances 32 B (8 tf32 / 16 fp16) per instruction
-        const uint64_t ad = make_wgmma_desc(sA + kk * 32, 16, 1024);
-        const uint64_t bd = make_wgmma_desc(sB + kk * 32, 16, 1024);
-        if (F16) wgmma_f16_n128<0, 0>(acc, ad, bd, 1);
-        else wgmma_tf32_n128(acc, ad, bd, 1);
+      for (int i = 0; i < 64; ++i) acc_x[i] = 0.f;
+      wgmma_fence_acc(acc);
+      wgmma_fence_acc(acc_x);
+      int prev = -1;
+      for (int ks = 0; ks < ksteps; ++ks, ++it) {
+        const int s = it % kStages;
+        mbar_wait(&L.full_bar[s], (it / kStages) & 1);
+        const uint32_t sAhi = smem_u32(L.stages + s * kStageBytes) + g * 64 * ROW_BYTES;  // this warpgroup's 64 rows of A
+        const uint32_t sAlo = sAhi + A_BYTES;
+        const uint32_t sBhi = smem_u32(L.stages + s * kStageBytes) + 2 * A_BYTES, sBlo = sBhi + A_BYTES;
+        wgmma_fence();
+        // K-major, 64 B swizzle: 8-row groups are 512 B apart (SBO); K advances 32 B (16 fp16) per instruction
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk)
+          wgmma_f16_n128<0, 0>(acc, make_wgmma_desc<2>(sAhi + kk * 32, 16, 512), make_wgmma_desc<2>(sBhi + kk * 32, 16, 512), 1);
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          wgmma_f16_n128<0, 0>(acc_x, make_wgmma_desc<2>(sAlo + kk * 32, 16, 512), make_wgmma_desc<2>(sBhi + kk * 32, 16, 512), 1);
+          wgmma_f16_n128<0, 0>(acc_x, make_wgmma_desc<2>(sAhi + kk * 32, 16, 512), make_wgmma_desc<2>(sBlo + kk * 32, 16, 512), 1);
+        }
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+        }
+        prev = s;
       }
-      wgmma_commit();
-      if (prev >= 0) {
-        wgmma_wait<1>();
-        if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      wgmma_fence_acc(acc_x);
+      if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = __fadd_rn(acc[i], acc_x[i]);
+    } else {
+      wgmma_fence_acc(acc);
+      int prev = -1;
+      for (int ks = 0; ks < ksteps; ++ks, ++it) {
+        const int s = it % kStages;
+        mbar_wait(&L.full_bar[s], (it / kStages) & 1);
+        const uint32_t sA = smem_u32(L.stages + s * kStageBytes) + g * 64 * 128;  // this warpgroup's 64 rows of A
+        const uint32_t sB = smem_u32(L.stages + s * kStageBytes) + A_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          // K-major, 128 B swizzle: 8-row groups are 1024 B apart (SBO); K advances 32 B (8 tf32 / 16 fp16) per instruction
+          const uint64_t ad = make_wgmma_desc(sA + kk * 32, 16, 1024);
+          const uint64_t bd = make_wgmma_desc(sB + kk * 32, 16, 1024);
+          if (F16) wgmma_f16_n128<0, 0>(acc, ad, bd, 1);
+          else wgmma_tf32_n128(acc, ad, bd, 1);
+        }
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+        }
+        prev = s;
       }
-      prev = s;
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
     }
-    wgmma_wait<0>();
-    wgmma_fence_acc(acc);
-    if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
 
     auto to_raw = [&](float* rw, int slab) { wgmma_acc_to_raw(acc, rw, slab, w, lane); };
     auto chunk_fn = [&](float (&o)[32], int slab, int r_off, int c_off) {
@@ -635,7 +747,9 @@ int make_tmap_any(CUtensorMap* out, const void* base, int64_t rows, int64_t cols
   cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * static_cast<cuuint64_t>(elem_bytes)};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1u, 1u};
-  const CUtensorMapSwizzle sw = swizzle == TMAP_SW128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE;
+  const CUtensorMapSwizzle sw = swizzle == TMAP_SW128  ? CU_TENSOR_MAP_SWIZZLE_128B
+                                : swizzle == TMAP_SW64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                       : CU_TENSOR_MAP_SWIZZLE_NONE;
   CUresult r = fn(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -653,28 +767,29 @@ static cudaError_t set_smem_attr_once(K kern, bool& done) {
   return cudaSuccess;
 }
 
-template <bool F16>
+template <bool F16, bool SPLIT>
 static cudaError_t launch_gram_t(const GramLaunch& g, cudaStream_t st) {
-  if (g.chunk_rows % GramCfg<F16>::SR != 0) return cudaErrorInvalidValue;
-  auto kern = gram_tn_kernel<F16>;
+  if (g.chunk_rows % GramCfg<F16, SPLIT>::SR != 0) return cudaErrorInvalidValue;
+  auto kern = gram_tn_kernel<F16, SPLIT>;
   static bool attr_done = false;
   cudaError_t e = set_smem_attr_once(kern, attr_done);
   if (e != cudaSuccess) return e;
   const int chunks = (g.rows + g.chunk_rows - 1) / g.chunk_rows;
   const unsigned grid = static_cast<unsigned>(chunks) * static_cast<unsigned>(g.num_tiles);
   if (grid == 0) return cudaSuccess;
-  kern<<<grid, kThreads, kSmemBytes, st>>>(g.tmA, g.tmB0, g.tmB1, g.tmOut0, g.tmOut1, g.tiles, g.num_tiles, g.rows, g.chunk_rows,
-                                           g.n_valid0, g.n_valid1);
+  kern<<<grid, kThreads, kSmemBytes, st>>>(g.tmA, g.tmB0, g.tmB1, g.tmOut0, g.tmOut1, SPLIT ? g.tmAlo : g.tmA, SPLIT ? g.tmB0lo : g.tmB0,
+                                           SPLIT ? g.tmB1lo : g.tmB1, g.tiles, g.num_tiles, g.rows, g.chunk_rows, g.n_valid0, g.n_valid1);
   return cudaGetLastError();
 }
 
 cudaError_t launch_gram(const GramLaunch& g, cudaStream_t st) {
-  return g.f16 ? launch_gram_t<true>(g, st) : launch_gram_t<false>(g, st);
+  if (g.split) return g.f16 ? launch_gram_t<true, true>(g, st) : cudaErrorInvalidValue;
+  return g.f16 ? launch_gram_t<true, false>(g, st) : launch_gram_t<false, false>(g, st);
 }
 
-template <int EPI, bool F16, int OUT16>
+template <int EPI, bool F16, int OUT16, bool SPLIT = false>
 static cudaError_t launch_km_t(const KmLaunch& k, cudaStream_t st) {
-  auto kern = gemm_kmajor_kernel<EPI, F16, OUT16>;
+  auto kern = gemm_kmajor_kernel<EPI, F16, OUT16, SPLIT>;
   static bool attr_done = false;
   cudaError_t e = set_smem_attr_once(kern, attr_done);
   if (e != cudaSuccess) return e;
@@ -683,11 +798,13 @@ static cudaError_t launch_km_t(const KmLaunch& k, cudaStream_t st) {
   const long long total = static_cast<long long>(m_tiles) * n_tiles;
   if (total == 0) return cudaSuccess;
   const unsigned grid = static_cast<unsigned>(total < k.num_sms ? total : k.num_sms);
-  kern<<<grid, kThreads, kSmemBytes, st>>>(k.tmA, k.tmB, k.tmOut, OUT16 == 2 ? k.tmOut2 : k.tmOut, k.p);
+  kern<<<grid, kThreads, kSmemBytes, st>>>(k.tmA, k.tmB, k.tmOut, OUT16 == 2 ? k.tmOut2 : k.tmOut, SPLIT ? k.tmAlo : k.tmA,
+                                           SPLIT ? k.tmBlo : k.tmB, k.p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_kmajor(const KmLaunch& k, cudaStream_t st) {
+  if (k.split) return (k.f16 && k.epi == EPI_UPDATE) ? launch_km_t<EPI_UPDATE, true, 0, true>(k, st) : cudaErrorInvalidValue;
   if (k.epi == EPI_POOL) return k.f16 ? launch_km_t<EPI_POOL, true, 0>(k, st) : cudaErrorInvalidValue;
   if (k.f16 && k.epi == EPI_APPLY) return launch_km_t<EPI_APPLY, true, 0>(k, st);
   if (k.f16 && k.epi == EPI_UPDATE) return launch_km_t<EPI_UPDATE, true, 0>(k, st);
