@@ -209,6 +209,30 @@ KS_API int32_t ks_model_cost(int64_t ctx, int64_t model, int64_t features, int64
                       int64_t labels, double lambda, double* out_cost);
 KS_API int32_t ks_model_destroy(int64_t ctx, int64_t model);
 
+/* ---- Gaussian-kernel ridge regression -------------------------------------------------------
+ * GaussianKernelGenerator(gamma).fit(train) (K/nodes/learning/KernelGenerator.scala:121-176): K(x, y) = exp(-gamma |x - y|^2).
+ * Collective: every rank passes its training rows; the kernel object holds ALL training rows on every rank (gathered in rank
+ * order: the global row order of the fit and of the model blocks), shifted by their exact fp64 column mean.
+ * gamma must be finite and > 0. */
+KS_API int32_t ks_gaussian_kernel_create(int64_t ctx, int64_t x_train, double gamma, int64_t* out_kernel);
+/* KernelMatrix(colIdxs) (K/nodes/learning/KernelMatrix.scala): K(x, x_train[col0, col0 + cols)) as a new (x rows x cols) fp32
+ * matrix; x holds raw input rows with the training column count. */
+KS_API int32_t ks_gaussian_kernel_block(int64_t ctx, int64_t kernel, int64_t x, int64_t col0, int64_t cols, int64_t* out_m);
+/* training rows over all ranks (the columns of the kernel matrix) and their width; either pointer may be NULL */
+KS_API int32_t ks_gaussian_kernel_shape(int64_t ctx, int64_t kernel, int64_t* n_train, int64_t* dim);
+KS_API int32_t ks_gaussian_kernel_destroy(int64_t ctx, int64_t kernel);
+/* KernelRidgeRegression(kernelGenerator, lambda, blockSize, numEpochs, blockPermuter).fit (K/nodes/learning/
+ * KernelRidgeRegression.scala:116-200): block Gauss-Seidel on (K + lambda I) W = Y over contiguous blocks of training rows, no
+ * centring, no intercept.  labels: this rank's rows.  block_order (num_epochs x n_blocks, each row a permutation of the blocks)
+ * or NULL for the sequential order.  Returns a kernel model (KernelBlockLinearMapper): ks_model_apply / _apply_argmax /
+ * _confusion_matrix take the raw input rows as `features` (x_in = 0, no rfs); ks_model_save / _cost / _apply_partial reject it.
+ * K_BB + lambda I not positive definite (lambda = 0 with repeated rows): KS_ERR_NOT_SPD on every rank.  Collective. */
+KS_API int32_t ks_krr_fit(int64_t ctx, int64_t kernel, int64_t labels, double lambda, int32_t block_size, int32_t num_epochs,
+                          const int32_t* block_order_or_null, int64_t* out_model);
+/* new KernelBlockLinearMapper(xs, blockSize, kernelTransformer, nTrain): block_rows must sum to the kernel's training rows. */
+KS_API int32_t ks_kernel_model_from_host(int64_t ctx, int64_t kernel, const double* const* xs_colmajor, const int64_t* block_rows,
+                                         int32_t n_blocks, int64_t k, int32_t block_size, int64_t* out_model);
+
 /* ---- on-disk formats at the edges of the path (host code; need no context) -----------------
  * Headerless CSV of doubles (K/loaders/CsvDataLoader.scala:28-30): ks_csv_dims counts rows and the fields of the first row;
  * ks_csv_read_* parse into a caller-owned row-major buffer (pinned memory makes the following upload asynchronous), split by

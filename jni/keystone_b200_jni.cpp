@@ -269,3 +269,57 @@ JFN(jlong, modelLoad)(JNIEnv* env, jobject, jlong ctx, jstring path) {
   return ok(env, ctx, rc) ? h : 0;
 }
 JFN(void, modelDestroy)(JNIEnv*, jobject, jlong ctx, jlong model) { ks_model_destroy(ctx, model); }
+
+// ---- Gaussian-kernel ridge regression
+JFN(jlong, gaussianKernelCreate)(JNIEnv* env, jobject, jlong ctx, jlong xTrain, jdouble gamma) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_gaussian_kernel_create(ctx, xTrain, gamma, &h)) ? h : 0;
+}
+JFN(jlong, gaussianKernelBlock)(JNIEnv* env, jobject, jlong ctx, jlong kernel, jlong x, jlong col0, jlong cols) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_gaussian_kernel_block(ctx, kernel, x, col0, cols, &h)) ? h : 0;
+}
+JFN(jlong, gaussianKernelNumTrain)(JNIEnv* env, jobject, jlong ctx, jlong kernel) {
+  int64_t n = 0;
+  return ok(env, ctx, ks_gaussian_kernel_shape(ctx, kernel, &n, nullptr)) ? n : 0;
+}
+JFN(void, gaussianKernelDestroy)(JNIEnv*, jobject, jlong ctx, jlong kernel) { ks_gaussian_kernel_destroy(ctx, kernel); }
+JFN(jlong, krrFit)(JNIEnv* env, jobject, jlong ctx, jlong kernel, jlong labels, jdouble lambda, jint blockSize, jint numEpochs,
+                   jintArray blockOrderOrNull) {
+  int64_t h = 0;
+  jint* order = blockOrderOrNull ? env->GetIntArrayElements(blockOrderOrNull, nullptr) : nullptr;
+  if (blockOrderOrNull && !order) return 0;  // OutOfMemoryError pending
+  const int32_t rc = ks_krr_fit(ctx, kernel, labels, lambda, blockSize, numEpochs, reinterpret_cast<const int32_t*>(order), &h);
+  if (order) env->ReleaseIntArrayElements(blockOrderOrNull, order, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, kernelModelFromHost)(JNIEnv* env, jobject, jlong ctx, jlong kernel, jobjectArray xs, jlong k, jint blockSize) {
+  const jsize nb = env->GetArrayLength(xs);
+  int64_t h = 0;
+  enum { kMax = 1 << 16 };  // KernelBlockLinearMapper models have nTrain / blockSize blocks
+  if (nb <= 0 || nb > kMax || k <= 0) {
+    ok(env, ctx, KS_ERR_INVALID);
+    return 0;
+  }
+  static thread_local const double* wp[kMax];
+  static thread_local int64_t rows[kMax];
+  static thread_local jdoubleArray wa[kMax];
+  jsize got = 0;
+  bool fail = false;
+  for (; got < nb; ++got) {
+    wa[got] = static_cast<jdoubleArray>(env->GetObjectArrayElement(xs, got));
+    wp[got] = env->GetDoubleArrayElements(wa[got], nullptr);
+    rows[got] = env->GetArrayLength(wa[got]) / k;
+    if (!wp[got]) {
+      fail = true;
+      ++got;
+      break;
+    }
+  }
+  int32_t rc = KS_ERR_INVALID;
+  if (!fail) rc = ks_kernel_model_from_host(ctx, kernel, wp, rows, nb, k, blockSize, &h);
+  for (jsize j = 0; j < got; ++j)
+    if (wp[j]) env->ReleaseDoubleArrayElements(wa[j], const_cast<jdouble*>(wp[j]), JNI_ABORT);
+  if (fail) return 0;  // OutOfMemoryError already pending
+  return ok(env, ctx, rc) ? h : 0;
+}

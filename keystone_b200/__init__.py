@@ -13,7 +13,12 @@ from .nodes import (  # noqa: F401
     ClassLabelIndicatorsFromIntLabels,
     Convolver,
     CosineRandomFeatures,
+    GaussianKernelGenerator,
+    GaussianKernelTransformer,
     ImageVectorizer,
+    KernelBlockLinearMapper,
+    KernelMatrix,
+    KernelRidgeRegression,
     Pooler,
     SymmetricRectifier,
     cifar_bytes_to_matrix,

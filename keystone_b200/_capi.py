@@ -104,6 +104,12 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_model_destroy", i64, i64)
     sig("ks_model_save", i64, i64, C.c_char_p)
     sig("ks_model_load", i64, C.c_char_p, p_i64)
+    sig("ks_gaussian_kernel_create", i64, i64, f64, p_i64)
+    sig("ks_gaussian_kernel_block", i64, i64, i64, i64, i64, p_i64)
+    sig("ks_gaussian_kernel_shape", i64, i64, p_i64, p_i64)
+    sig("ks_gaussian_kernel_destroy", i64, i64)
+    sig("ks_krr_fit", i64, i64, i64, f64, i32, i32, C.c_void_p, p_i64)
+    sig("ks_kernel_model_from_host", i64, i64, pp_f64, p_i64, i32, i64, i32, p_i64)
     sig("ks_io_last_error", restype=C.c_char_p)
     sig("ks_csv_dims", C.c_char_p, p_i64, p_i64)
     sig("ks_csv_read_f64", C.c_char_p, C.c_void_p, i64, i64, i64)

@@ -76,13 +76,6 @@ NcclApi& nccl_api() {
   if (!fail.empty()) throw KsError{KS_ERR_NCCL, fail};
   return api;
 }
-#define KS_NCCL(call)                                                                                      \
-  do {                                                                                                     \
-    ncclResult_t r__ = (call);                                                                             \
-    if (r__ != ncclSuccess)                                                                                \
-      throw KsError{KS_ERR_NCCL, std::string(#call) + " failed: " + nccl_api().GetErrorString(r__)};      \
-  } while (0)
-
 // ------------------------------------------------------------------------------------ caching device-memory pool
 // Blocks are keyed by (device, size rounded up to 2 MiB); freed blocks are kept for reuse and released when the last
 // context is destroyed.  Buffers freed here may still be in use by work queued on the context's stream: every path that
@@ -1277,7 +1270,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
 }
 
 // ------------------------------------------------------------------------------------ apply
-static std::unique_ptr<Matrix> new_matrix(int64_t rows, int64_t cols) {
+std::unique_ptr<Matrix> new_matrix(int64_t rows, int64_t cols) {
   auto m = std::make_unique<Matrix>();
   m->rows = rows;
   m->cols = cols;
@@ -1509,6 +1502,7 @@ KS_API int32_t ks_ctx_destroy(int64_t ctx) {
   c->matrices.clear();
   c->rfs.clear();
   c->models.clear();
+  c->kernels.clear();
   c->convs.clear();
   c->tile_cache.clear();
   for (auto e : c->event_pool) cudaEventDestroy(e);
@@ -2089,6 +2083,15 @@ KS_API int32_t ks_model_host_view(int64_t ctx, int64_t model, int32_t j, const d
     if (intercept_ptr) *intercept_ptr = m.has_intercept ? reinterpret_cast<const double*>(h + m.host_b_off) : nullptr;
   });
 }
+// KernelBlockLinearMapper: applied to raw input rows (features) only
+static std::unique_ptr<Matrix> apply_kernel_model(Ctx& c, Model& m, int64_t features, int64_t x_in, int32_t n_rfs) {
+  if (x_in != 0 || n_rfs != 0 || features == 0)
+    throw KsError{KS_ERR_INVALID, "a kernel model is applied to raw input rows: pass them as features, without x_in / rfs"};
+  return kernel_model_apply(c, m, c.matrix(features));
+}
+static void reject_kernel_model(const Model& m, const char* what) {
+  if (m.kernel) throw KsError{KS_ERR_INVALID, std::string(what) + " is not available for kernel models (KernelBlockLinearMapper)"};
+}
 // Flat model file (little endian): "KSB2MDL1", int32 block_size, int32 n_blocks, int64 k, int32 has_mean, int32 has_intercept,
 // int64 rows[n_blocks], then per block W (rows x k fp64, column-major) [+ rows means], then k intercepts.  Replaces the
 // Java-serialised FittedPipeline of the reference (K/workflow/FittedPipeline.scala:18-22) for the BlockLinearMapper stage.
@@ -2096,6 +2099,7 @@ KS_API int32_t ks_model_save(int64_t ctx, int64_t model, const char* path) {
   return guard(ctx, [&](Ctx& c) {
     if (!path) throw KsError{KS_ERR_INVALID, "null path"};
     Model& m = c.model(model);
+    reject_kernel_model(m, "save (kernel models hold the training rows and are not persisted)");
     ensure_host_mirror(c, m);
     FILE* f = fopen(path, "wb");
     if (!f) throw KsError{KS_ERR_INVALID, std::string("cannot open ") + path + " for writing"};
@@ -2183,6 +2187,10 @@ KS_API int32_t ks_model_get_intercept(int64_t ctx, int64_t model, double* b_out,
 KS_API int32_t ks_model_apply(int64_t ctx, int64_t model, int64_t features, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int64_t* out) {
   return guard(ctx, [&](Ctx& c) {
     if (!out) throw KsError{KS_ERR_INVALID, "null output"};
+    if (c.model(model).kernel) {
+      *out = c.add(apply_kernel_model(c, c.model(model), features, x_in, n_rfs));
+      return;
+    }
     FeatSrc src;
     make_feat_src(c, features, x_in, rfs, n_rfs, src, c.precision);
     *out = c.add(apply_model(c, c.model(model), src, -1, true, c.precision));
@@ -2192,6 +2200,7 @@ KS_API int32_t ks_model_apply_partial(int64_t ctx, int64_t model, int64_t featur
                                int32_t last_block, int64_t* out) {
   return guard(ctx, [&](Ctx& c) {
     if (!out) throw KsError{KS_ERR_INVALID, "null output"};
+    reject_kernel_model(c.model(model), "apply_partial");
     FeatSrc src;
     make_feat_src(c, features, x_in, rfs, n_rfs, src, c.precision);
     *out = c.add(apply_model(c, c.model(model), src, last_block, true, c.precision));
@@ -2201,9 +2210,14 @@ KS_API int32_t ks_model_apply_argmax(int64_t ctx, int64_t model, int64_t feature
                               int32_t* host_out) {
   return guard(ctx, [&](Ctx& c) {
     if (!host_out) throw KsError{KS_ERR_INVALID, "null output"};
-    FeatSrc src;
-    make_feat_src(c, features, x_in, rfs, n_rfs, src, c.precision);
-    auto y = apply_model(c, c.model(model), src, -1, true, c.precision);
+    std::unique_ptr<Matrix> y;
+    if (c.model(model).kernel) {
+      y = apply_kernel_model(c, c.model(model), features, x_in, n_rfs);
+    } else {
+      FeatSrc src;
+      make_feat_src(c, features, x_in, rfs, n_rfs, src, c.precision);
+      y = apply_model(c, c.model(model), src, -1, true, c.precision);
+    }
     DevBuf idx;
     idx.alloc(sizeof(int32_t) * static_cast<size_t>(std::max<int64_t>(y->rows, 1)));
     launch_argmax_rows(y->d, y->ld, y->rows, static_cast<int>(y->cols), idx.as<int32_t>(), c.st);
@@ -2218,11 +2232,17 @@ KS_API int32_t ks_model_confusion_matrix(int64_t ctx, int64_t model, int64_t fea
     if (!out_counts) throw KsError{KS_ERR_INVALID, "null output"};
     Model& m = c.model(model);
     Matrix& L = c.matrix(labels);
-    FeatSrc src;
-    make_feat_src(c, features, x_in, rfs, n_rfs, src, c.precision);
-    if (L.rows != src.n_rows || L.cols != m.k) throw KsError{KS_ERR_INVALID, "labels shape mismatch"};
+    std::unique_ptr<Matrix> y;
+    if (m.kernel) {
+      if (features == 0 || L.rows != c.matrix(features).rows || L.cols != m.k) throw KsError{KS_ERR_INVALID, "labels shape mismatch"};
+      y = apply_kernel_model(c, m, features, x_in, n_rfs);
+    } else {
+      FeatSrc src;
+      make_feat_src(c, features, x_in, rfs, n_rfs, src, c.precision);
+      if (L.rows != src.n_rows || L.cols != m.k) throw KsError{KS_ERR_INVALID, "labels shape mismatch"};
+      y = apply_model(c, m, src, -1, true, c.precision);
+    }
     const int k = static_cast<int>(m.k);
-    auto y = apply_model(c, m, src, -1, true, c.precision);
     DevBuf pred, act, counts;
     pred.alloc(sizeof(int32_t) * static_cast<size_t>(std::max<int64_t>(y->rows, 1)));
     act.alloc(pred.bytes);
@@ -2245,6 +2265,7 @@ KS_API int32_t ks_model_cost(int64_t ctx, int64_t model, int64_t features, int64
   return guard(ctx, [&](Ctx& c) {
     if (!out_cost) throw KsError{KS_ERR_INVALID, "null output"};
     Model& m = c.model(model);
+    reject_kernel_model(m, "computeCost");
     Matrix& L = c.matrix(labels);
     FeatSrc src;
     make_feat_src(c, features, x_in, rfs, n_rfs, src, c.precision);
@@ -2272,6 +2293,53 @@ KS_API int32_t ks_model_cost(int64_t ctx, int64_t model, int64_t features, int64
 KS_API int32_t ks_model_destroy(int64_t ctx, int64_t model) {
   return guard(ctx, [&](Ctx& c) {
     if (!c.models.erase(model)) throw KsError{KS_ERR_HANDLE, "unknown model handle"};
+  });
+}
+
+// ---------------------------------------------------------------- Gaussian kernel ridge regression (krr.cu)
+static std::shared_ptr<GaussKernel> find_kernel(Ctx& c, int64_t h) {
+  auto it = c.kernels.find(h);
+  if (it == c.kernels.end()) throw KsError{KS_ERR_HANDLE, "unknown Gaussian kernel handle " + std::to_string(h)};
+  return it->second;
+}
+KS_API int32_t ks_gaussian_kernel_create(int64_t ctx, int64_t x_train, double gamma, int64_t* out_kernel) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_kernel) throw KsError{KS_ERR_INVALID, "null out_kernel"};
+    *out_kernel = gaussian_kernel_create(c, c.matrix(x_train), gamma);
+  });
+}
+KS_API int32_t ks_gaussian_kernel_block(int64_t ctx, int64_t kernel, int64_t x, int64_t col0, int64_t cols, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    auto K = find_kernel(c, kernel);
+    *out_m = c.add(gaussian_kernel_block(c, *K, c.matrix(x), col0, cols));
+  });
+}
+KS_API int32_t ks_gaussian_kernel_shape(int64_t ctx, int64_t kernel, int64_t* n_train, int64_t* dim) {
+  return guard(ctx, [&](Ctx& c) {
+    auto K = find_kernel(c, kernel);
+    if (n_train) *n_train = K->n;
+    if (dim) *dim = K->d;
+  });
+}
+KS_API int32_t ks_gaussian_kernel_destroy(int64_t ctx, int64_t kernel) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!c.kernels.erase(kernel)) throw KsError{KS_ERR_HANDLE, "unknown Gaussian kernel handle"};
+  });
+}
+KS_API int32_t ks_krr_fit(int64_t ctx, int64_t kernel, int64_t labels, double lambda, int32_t block_size, int32_t num_epochs,
+                          const int32_t* block_order_or_null, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    auto K = find_kernel(c, kernel);
+    *out_model = fit_krr(c, K, c.matrix(labels), lambda, block_size, num_epochs, block_order_or_null);
+  });
+}
+KS_API int32_t ks_kernel_model_from_host(int64_t ctx, int64_t kernel, const double* const* xs_colmajor, const int64_t* block_rows,
+                                         int32_t n_blocks, int64_t k, int32_t block_size, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    *out_model = kernel_model_from_host(c, find_kernel(c, kernel), xs_colmajor, block_rows, n_blocks, k, block_size);
   });
 }
 

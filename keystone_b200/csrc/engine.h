@@ -109,7 +109,22 @@ struct ConvPool {
   bool has_means = false;
 };
 
+// GaussianKernelGenerator.fit (K/nodes/learning/KernelGenerator.scala:121-176): the whole training X, replicated on every rank,
+// shifted by its exact column mean m (distances are shift-invariant; the shift removes the cancellation in
+// |x|^2 + |y|^2 - 2 x.y for uncentred data), with its split-operand copies and squared norms.  krr.cu, DESIGN.md section 13.
+struct GaussKernel {
+  double gamma = 0;
+  int64_t n = 0, d = 0, ld = 0, ld3 = 0;
+  int64_t row_off = 0, n_loc = 0;  // this rank's training rows [row_off, row_off + n_loc) in the global order
+  DevBuf xs;     // fp32 [n][ld]: x - m
+  DevBuf mean;   // fp64 [d]: m
+  DevBuf xb3;    // fp16 [n][ld3]: [hi | hi | lo] of 2^e (x - m), the column-side operand of the generation GEMM
+  DevBuf norms;  // fp32 [n]: sum of ((hi + lo) 2^-e)^2, the squared norm of exactly the values the pair represents
+  DevBuf scale;  // fp32 [2]: 2^e, 2^-e
+};
+
 struct Model {  // BlockLinearMapper state (K/nodes/learning/BlockLinearMapper.scala:22-33)
+  std::shared_ptr<GaussKernel> kernel;  // KernelBlockLinearMapper (K/nodes/learning/KernelBlockLinearMapper.scala): the training rows
   int block_size = 0;
   int64_t k = 0;
   std::vector<int64_t> brows;
@@ -148,6 +163,12 @@ struct NcclApi {
 };
 SolverApi& solver_api();  // throws KsError if libcusolver cannot be loaded
 NcclApi& nccl_api();      // throws KsError if libnccl cannot be loaded
+#define KS_NCCL(call)                                                                                      \
+  do {                                                                                                     \
+    ncclResult_t r__ = (call);                                                                             \
+    if (r__ != ncclSuccess)                                                                                \
+      throw ::ks::KsError{KS_ERR_NCCL, std::string(#call) + " failed: " + ::ks::nccl_api().GetErrorString(r__)}; \
+  } while (0)
 
 enum Phase { PH_FEATURIZE = 0, PH_GRAM, PH_ALLREDUCE, PH_SOLVE, PH_UPDATE, PH_OTHER, PH_COUNT };
 
@@ -209,6 +230,7 @@ struct Ctx {
   std::unordered_map<int64_t, std::unique_ptr<CosRF>> rfs;
   std::unordered_map<int64_t, std::unique_ptr<Model>> models;
   std::unordered_map<int64_t, std::unique_ptr<ConvPool>> convs;
+  std::unordered_map<int64_t, std::shared_ptr<GaussKernel>> kernels;
   std::map<std::vector<int>, std::unique_ptr<DevBuf>> tile_cache;
   // phase timing of the current fit
   struct Span { int phase; cudaEvent_t a, b; int stream; };
@@ -296,5 +318,15 @@ int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double l
 void model_alloc_host(Model& m);
 void model_block_to_host(Model& m, int j, cudaStream_t s);
 void model_intercept_to_host(Model& m, cudaStream_t s);
+
+// Gaussian-kernel ridge regression (krr.cu)
+std::unique_ptr<Matrix> new_matrix(int64_t rows, int64_t cols);
+int64_t gaussian_kernel_create(Ctx& c, Matrix& X, double gamma);  // collective
+std::unique_ptr<Matrix> gaussian_kernel_block(Ctx& c, const GaussKernel& K, Matrix& x, int64_t col0, int64_t cols);
+int64_t fit_krr(Ctx& c, const std::shared_ptr<GaussKernel>& K, Matrix& Y, double lam, int bs, int epochs,
+                const int32_t* order_or_null);  // collective
+std::unique_ptr<Matrix> kernel_model_apply(Ctx& c, Model& md, Matrix& x);
+int64_t kernel_model_from_host(Ctx& c, const std::shared_ptr<GaussKernel>& K, const double* const* xs, const int64_t* block_rows,
+                               int32_t n_blocks, int64_t k, int32_t block_size);
 
 }  // namespace ks

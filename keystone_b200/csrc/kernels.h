@@ -9,7 +9,7 @@ namespace ks {
 static constexpr int kGramStageRows = 32;  // rows per TMA stage of the Gram kernel
 static constexpr int kPadCols = 32;        // every device matrix has ld % 32 == 0 (128 B rows)
 
-enum { EPI_COS = 0, EPI_UPDATE = 1, EPI_APPLY = 2, EPI_POOL = 3 };
+enum { EPI_COS = 0, EPI_UPDATE = 1, EPI_APPLY = 2, EPI_POOL = 3, EPI_RBF = 4 };
 
 struct GramTile {
   int m_blk;  // 128-wide block of A's columns
@@ -45,6 +45,10 @@ struct KmParams {
   int patches_per_image = 0, n_pools = 0;
   float pool_alpha = 0.f;
   int* tile_counter = nullptr;  // persistent single-CTA kernel: zeroed device counter the CTAs draw their tiles from (null: static stride)
+  // EPI_RBF (Gaussian kernel block): out = exp(-gamma * max(0, row_vec[m] + vec0[n] - 2 acc)), row_vec / vec0 the squared norms
+  // of the rows of A / B
+  const float* row_vec = nullptr;
+  float gamma = 0.f;
   int M, N, K;
   int flags;  // KM_FLAG_NO_ROUND: EPI_COS keeps fp32;  KM_FLAG_REDUCE: add into the output instead of overwriting it
 };
@@ -58,7 +62,7 @@ struct KmLaunch {
   int num_sms;
   int f16 = 0;   // 1: fp16 operands
   int split = 0; // 1 (EPI_UPDATE, f16 only): operands are fp16 pairs, one pass computes A_hi B_hi^T + A_lo B_hi^T + A_hi B_lo^T
-  int out16 = 0; // EPI_COS: 1 = the slab is written as fp16 (tmOut: {32, 32} fp16 boxes, no swizzle); 2 = as the fp16 pair hi + lo
+  int out16 = 0; // EPI_COS (EPI_RBF: 2 only): 1 = the slab is written as fp16 (tmOut: {32, 32} fp16 boxes, no swizzle); 2 = as the fp16 pair hi + lo
                  // of the unrounded value (tmOut, tmOut2)
 };
 

@@ -11,6 +11,7 @@
 //                       EPI_UPDATE  R   += -acc + cbias                      (BlockWeightedLeastSquares.scala:287-290)
 //                       EPI_APPLY   Y [+]= acc + cbias                       (BlockLinearMapper.scala:55-70)
 //                       EPI_POOL    Convolver -> SymmetricRectifier -> sum Pooler (Convolver.scala, Pooler.scala)
+//                       EPI_RBF     out  = exp(-gamma (n_i + n_j - 2 acc))   (KernelGenerator.scala:160-176)
 //
 // Both kernels are 128 x 128 output tiles on 384 threads: warpgroup 0 issues the TMA loads of a 4-stage mbarrier ring,
 // warpgroups 1 and 2 each own 64 output rows (one m64n128 wgmma accumulator, 64 fp32 registers per thread) and run the
@@ -423,6 +424,11 @@ __device__ __forceinline__ void km_chunk(const KmParams& p, const CUtensorMap* t
   } else if (EPI == EPI_APPLY) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = v0s[i] + a[i] * ascale;
+  } else if (EPI == EPI_RBF) {
+    // squared distance from the norms and the cross product; full-precision expf (the value is stored as a 21-bit pair)
+    const float ni = row0 + lane < p.M ? __ldg(p.row_vec + row0 + lane) : 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = expf(-p.gamma * fmaxf(0.f, ni + v0s[i] - 2.f * a[i] * ascale));
   }
   if (EPI == EPI_POOL) {
     // Convolver -> SymmetricRectifier -> sum Pooler: the chunk (32 patch rows x 32 filters) is transposed through the staging
@@ -806,6 +812,7 @@ static cudaError_t launch_km_t(const KmLaunch& k, cudaStream_t st) {
 cudaError_t launch_kmajor(const KmLaunch& k, cudaStream_t st) {
   if (k.split) return (k.f16 && k.epi == EPI_UPDATE) ? launch_km_t<EPI_UPDATE, true, 0, true>(k, st) : cudaErrorInvalidValue;
   if (k.epi == EPI_POOL) return k.f16 ? launch_km_t<EPI_POOL, true, 0>(k, st) : cudaErrorInvalidValue;
+  if (k.epi == EPI_RBF) return (k.f16 && k.out16 == 2) ? launch_km_t<EPI_RBF, true, 2>(k, st) : cudaErrorInvalidValue;
   if (k.f16 && k.epi == EPI_APPLY) return launch_km_t<EPI_APPLY, true, 0>(k, st);
   if (k.f16 && k.epi == EPI_UPDATE) return launch_km_t<EPI_UPDATE, true, 0>(k, st);
   if (k.out16 == 2 && k.epi == EPI_COS) return k.f16 ? launch_km_t<EPI_COS, true, 2>(k, st) : cudaErrorInvalidValue;

@@ -632,6 +632,162 @@ class LeastSquaresEstimator(LabelEstimator, WeightedNode):
         return BlockLeastSquaresEstimator(1000, 3, self.lam, ctx=ds.ctx).fit(ds, lb)
 
 
+# ------------------------------------------------------------------------------------------ Gaussian-kernel ridge regression
+class _KernelHandle:
+    def __init__(self, ctx: Context, handle: int):
+        self.ctx, self.handle = ctx, handle
+
+    def __del__(self):
+        try:
+            if self.handle and self.ctx.handle:
+                lib().ks_gaussian_kernel_destroy(self.ctx.handle, self.handle)
+        except Exception:
+            pass
+
+
+def _device_rows(ctx: Optional[Context], data) -> DeviceMatrix:
+    ds = _as_dataset(ctx, data)
+    return ds if isinstance(ds, DeviceMatrix) else ds.materialize()
+
+
+class GaussianKernelGenerator(Estimator):
+    """``new GaussianKernelGenerator(gamma, cacheKernel)`` (K/nodes/learning/KernelGenerator.scala:36-44):
+    K(x, y) = exp(-gamma |x - y|^2).  ``cache_kernel`` is accepted for API parity and has no effect: kernel blocks are
+    regenerated on the device whenever they are needed."""
+
+    def __init__(self, gamma: float, cache_kernel: bool = False, ctx: Optional[Context] = None):
+        gamma = float(gamma)
+        if not (gamma > 0.0 and math.isfinite(gamma)):
+            raise ValueError("gamma must be finite and > 0")
+        self.gamma, self.cache_kernel, self.ctx = gamma, cache_kernel, ctx
+
+    def fit(self, train) -> "GaussianKernelTransformer":
+        """Collective with several ranks: every rank passes its training rows; the transformer holds all of them."""
+        x = _device_rows(self.ctx, train)
+        h = C.c_int64(0)
+        check(x.ctx.handle, lib().ks_gaussian_kernel_create(x.ctx.handle, x.handle, self.gamma, C.byref(h)))
+        return GaussianKernelTransformer(x.ctx, h.value, self.gamma)
+
+
+class GaussianKernelTransformer(Transformer):
+    """The fitted kernel (KernelGenerator.scala:84-119): the training rows of every rank, in rank order."""
+
+    def __init__(self, ctx: Context, handle: int, gamma: float):
+        self.ctx, self.handle, self.gamma = ctx, handle, gamma
+        self._owner = _KernelHandle(ctx, handle)
+        n, d = C.c_int64(0), C.c_int64(0)
+        check(ctx.handle, lib().ks_gaussian_kernel_shape(ctx.handle, handle, C.byref(n), C.byref(d)))
+        self.n_train, self.dim = n.value, d.value   # training rows over all ranks, their width
+
+    def block(self, data, col0: int, cols: int) -> DeviceMatrix:
+        """K(data, training rows [col0, col0 + cols)) as a device matrix."""
+        x = _device_rows(self.ctx, data)
+        h = C.c_int64(0)
+        check(self.ctx.handle, lib().ks_gaussian_kernel_block(self.ctx.handle, self.handle, x.handle, int(col0), int(cols), C.byref(h)))
+        return DeviceMatrix(self.ctx, h.value, x.rows, int(cols))
+
+    def apply(self, data):
+        """A dataset gives its KernelMatrix (lazy); a 1-D vector gives its kernel row against every training row."""
+        if isinstance(data, np.ndarray) and data.ndim == 1:
+            return self.block(np.asarray(data, dtype=np.float64)[None, :], 0, self.n_train).to_numpy()[0]
+        return KernelMatrix(self, _device_rows(self.ctx, data))
+
+
+class KernelMatrix:
+    """BlockKernelMatrix (K/nodes/learning/KernelMatrix.scala:50-95): column blocks of K(data, training rows), generated on the
+    device when asked for.  Column blocks are contiguous ranges of training rows."""
+
+    def __init__(self, transformer: GaussianKernelTransformer, data: DeviceMatrix):
+        self.transformer, self.data = transformer, data
+
+    @staticmethod
+    def _range(idxs: Sequence[int]):
+        idx = np.asarray(list(idxs), dtype=np.int64)
+        if idx.size == 0 or np.any(np.diff(idx) != 1):
+            raise ValueError("column indices must be a non-empty contiguous ascending range")
+        return int(idx[0]), int(idx.size)
+
+    def __call__(self, col_idxs: Sequence[int]) -> DeviceMatrix:
+        c0, n = self._range(col_idxs)
+        return self.transformer.block(self.data, c0, n)
+
+    def diag_block(self, idxs: Sequence[int]) -> np.ndarray:
+        """K(data rows idxs, training rows idxs): the rows idxs of the column block idxs (this rank's data rows)."""
+        c0, n = self._range(idxs)
+        return self(idxs).to_numpy()[c0:c0 + n]
+
+    def unpersist(self, col_idxs: Sequence[int]) -> None:
+        """Nothing is cached."""
+
+
+class KernelBlockLinearMapper(BlockLinearMapper):
+    """``KernelBlockLinearMapper(model, blockSize, kernelTransformer, nTrain)`` (K/nodes/learning/KernelBlockLinearMapper.scala:
+    28-89): predictions sum_j K(x, X_j) W_j on raw input rows.  Kernel models are not persisted (save / compute_cost /
+    applyAndEvaluate raise)."""
+
+    def __init__(self, ctx: Context, handle: int, kernel_transformer: GaussianKernelTransformer):
+        super().__init__(ctx, handle)
+        self.kernel_transformer = kernel_transformer
+
+    @classmethod
+    def from_arrays(cls, ctx: Context, xs: Sequence[np.ndarray], block_size: int,  # type: ignore[override]
+                    kernel_transformer: GaussianKernelTransformer) -> "KernelBlockLinearMapper":
+        xs_f = [np.asfortranarray(np.asarray(x, dtype=np.float64)) for x in xs]
+        k = xs_f[0].shape[1]
+        ptrs = (C.POINTER(C.c_double) * len(xs_f))(*[x.ctypes.data_as(C.POINTER(C.c_double)) for x in xs_f])
+        rows = (C.c_int64 * len(xs_f))(*[x.shape[0] for x in xs_f])
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_kernel_model_from_host(ctx.handle, kernel_transformer.handle, ptrs, rows, len(xs_f), k, block_size,
+                                                           C.byref(h)))
+        return cls(ctx, h.value, kernel_transformer)
+
+    @property
+    def model(self) -> List[np.ndarray]:
+        return self.xs
+
+
+class KernelRidgeRegression(LabelEstimator):
+    """``new KernelRidgeRegression(kernelGenerator, lambda, blockSize, numEpochs, blockPermuter, blocksBeforeCheckpoint)``
+    (K/nodes/learning/KernelRidgeRegression.scala:37-84): block Gauss-Seidel on (K + lambda I) W = Y over contiguous blocks
+    of training rows, no centring, no intercept.
+
+    ``block_permuter``: a seed; each epoch visits the blocks in ``numpy.random.Generator(PCG64(seed)).permutation`` order (one
+    draw per epoch).  Scala's ``Random.shuffle`` stream is not reproduced.  ``blocks_before_checkpoint`` is accepted for API
+    parity and has no effect (there is no Spark lineage to truncate)."""
+
+    def __init__(self, kernel_generator: GaussianKernelGenerator, lam: float, block_size: int, num_epochs: int,
+                 block_permuter: Optional[int] = None, blocks_before_checkpoint: int = 25, ctx: Optional[Context] = None):
+        if int(block_size) < 1:
+            raise ValueError("block_size must be >= 1")
+        if int(num_epochs) < 1:
+            raise ValueError("num_epochs must be >= 1")
+        lam = float(lam)
+        if not (lam >= 0.0 and math.isfinite(lam)):
+            raise ValueError("lam must be finite and >= 0")
+        self.kernel_generator, self.lam, self.block_size, self.num_epochs = kernel_generator, lam, int(block_size), int(num_epochs)
+        self.block_permuter, self.blocks_before_checkpoint, self.ctx = block_permuter, blocks_before_checkpoint, ctx
+
+    def block_order(self, n_train: int) -> Optional[np.ndarray]:
+        if self.block_permuter is None:
+            return None
+        nb = -(-n_train // self.block_size)
+        rng = np.random.Generator(np.random.PCG64(self.block_permuter))
+        return np.stack([rng.permutation(nb) for _ in range(self.num_epochs)]).astype(np.int32)
+
+    def fit(self, data, labels) -> KernelBlockLinearMapper:
+        """Collective with several ranks (data and labels: this rank's rows)."""
+        x = _device_rows(self.ctx or self.kernel_generator.ctx, data)
+        ctx = x.ctx
+        lb = _device_rows(ctx, labels)
+        transformer = self.kernel_generator.fit(x)
+        order = self.block_order(transformer.n_train)
+        optr = None if order is None else np.ascontiguousarray(order).ctypes.data_as(C.c_void_p)
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_krr_fit(ctx.handle, transformer.handle, lb.handle, self.lam, self.block_size, self.num_epochs, optr,
+                                            C.byref(h)))
+        return KernelBlockLinearMapper(ctx, h.value, transformer)
+
+
 class StandardScalerModel(Transformer):
     """(x - mean) [/ std] as a LinearMapper-free node is out of the hot path; the fits above centre internally
     (BlockLinearMapper.scala:224-232).  Kept for API parity: holds the statistics a fitted model reports."""

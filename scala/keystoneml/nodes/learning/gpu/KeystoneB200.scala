@@ -44,6 +44,15 @@ class KeystoneB200 extends Serializable {
   @native def modelSave(ctx: Long, model: Long, path: String): Unit
   @native def modelLoad(ctx: Long, path: String): Long
   @native def modelDestroy(ctx: Long, model: Long): Unit
+
+  // Gaussian-kernel ridge regression (KernelGenerator / KernelRidgeRegression / KernelBlockLinearMapper)
+  @native def gaussianKernelCreate(ctx: Long, xTrain: Long, gamma: Double): Long
+  @native def gaussianKernelBlock(ctx: Long, kernel: Long, x: Long, col0: Long, cols: Long): Long
+  @native def gaussianKernelNumTrain(ctx: Long, kernel: Long): Long
+  @native def gaussianKernelDestroy(ctx: Long, kernel: Long): Unit
+  @native def krrFit(ctx: Long, kernel: Long, labels: Long, lambda: Double, blockSize: Int, numEpochs: Int,
+                     blockOrder: Array[Int]): Long
+  @native def kernelModelFromHost(ctx: Long, kernel: Long, xs: Array[Array[Double]], k: Long, blockSize: Int): Long
 }
 
 object KeystoneB200 {
