@@ -168,6 +168,16 @@ KS_API int32_t ks_blockwls_fit(int64_t ctx, int64_t features, int64_t x_in, cons
  * equations == one block covering all features.  has_lambda = 0 mirrors lambda = None. */
 KS_API int32_t ks_linear_map_fit(int64_t ctx, int64_t features, int64_t labels, int32_t has_lambda, double lambda,
                           int64_t* out_model);
+/* DenseLBFGSwithL2(LeastSquaresDenseGradient, fitIntercept, numCorrections, convergenceTol, numIterations, regParam).fit
+ * (K/nodes/learning/LBFGS.scala:135-173): minimises |A_c W - Y_c|^2 / (2N) + reg_param / 2 |W|^2 from W = 0 by L-BFGS with the
+ * last num_corrections pairs and the exact step along each direction (DESIGN.md section 14).  fit_intercept != 0 centres
+ * features and labels by their exact means and returns LinearMapper(W, label mean, feature means); 0 returns W alone.  Stops
+ * after num_iterations steps or, with convergence_tol > 0, when the loss or the gradient has converged; ks_last_fit_stats_json
+ * reports iterations, loss_history (f(W_0) .. f(W_T)) and stop_reason.  num_corrections and num_iterations must be >= 1,
+ * reg_param and convergence_tol finite and >= 0.  Returns an ordinary model handle.  Collective across ranks. */
+KS_API int32_t ks_lbfgs_fit(int64_t ctx, int64_t features, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int64_t labels,
+                            int32_t fit_intercept, int32_t num_corrections, double convergence_tol, int32_t num_iterations,
+                            double reg_param, int32_t precision_mode, int64_t* out_model);
 
 /* ---- BlockLinearMapper / LinearMapper state (K/nodes/learning/BlockLinearMapper.scala:22-33,
  * K/nodes/learning/LinearMapper.scala:18-22) ------------------------------------------------ */
@@ -252,6 +262,8 @@ KS_API int32_t ks_cifar_read(const char* path, uint8_t* images_out, int32_t* lab
  * JSON with per-phase device milliseconds of the last fit (featurize, gram, allreduce, solve, update),
  * kernel launch count and the algorithmic flop count. */
 KS_API int32_t ks_last_fit_stats_json(int64_t ctx, char* buf, int64_t buflen);
+/* bytes ks_last_fit_stats_json needs for the current JSON, terminating NUL included */
+KS_API int32_t ks_last_fit_stats_json_size(int64_t ctx, int64_t* out_bytes);
 /* number of kernels this library has launched on the context since creation */
 KS_API int32_t ks_ctx_launch_count(int64_t ctx, int64_t* out_count);
 

@@ -149,6 +149,14 @@ JFN(jlong, blockWlsFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong x
                                      numFeaturesOr0, precisionMode, &h);
   return ok(env, ctx, rc) ? h : 0;
 }
+JFN(jlong, lbfgsFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong xIn, jlongArray rfs, jlong labels, jboolean fitIntercept,
+                     jint numCorrections, jdouble convergenceTol, jint numIterations, jdouble regParam, jint precisionMode) {
+  int64_t h = 0;
+  LongArray r(env, rfs);
+  const int32_t rc = ks_lbfgs_fit(ctx, features, xIn, r.data(), r.n, labels, fitIntercept ? 1 : 0, numCorrections, convergenceTol,
+                                  numIterations, regParam, precisionMode, &h);
+  return ok(env, ctx, rc) ? h : 0;
+}
 JFN(jlong, linearMapFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong labels, jboolean hasLambda, jdouble lambda) {
   int64_t h = 0;
   return ok(env, ctx, ks_linear_map_fit(ctx, features, labels, hasLambda ? 1 : 0, lambda, &h)) ? h : 0;

@@ -13,6 +13,7 @@ from .nodes import (  # noqa: F401
     ClassLabelIndicatorsFromIntLabels,
     Convolver,
     CosineRandomFeatures,
+    DenseLBFGSwithL2,
     GaussianKernelGenerator,
     GaussianKernelTransformer,
     ImageVectorizer,
@@ -23,6 +24,7 @@ from .nodes import (  # noqa: F401
     SymmetricRectifier,
     cifar_bytes_to_matrix,
     images_to_matrix,
+    LeastSquaresDenseGradient,
     LeastSquaresEstimator,
     LinearMapEstimator,
     LinearMapper,

@@ -90,6 +90,7 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_blockls_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, i64, i32, p_i64)
     sig("ks_blockwls_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, f64, i64, i32, p_i64)
     sig("ks_linear_map_fit", i64, i64, i64, i32, f64, p_i64)
+    sig("ks_lbfgs_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, i32, f64, i32, p_i64)
     sig("ks_model_from_host", i64, pp_f64, p_i64, i32, i64, C.c_void_p, pp_f64, i32, p_i64)
     sig("ks_model_num_blocks", i64, i64, p_i32, p_i64, p_i32)
     sig("ks_model_block_rows", i64, i64, i32, p_i64)
@@ -117,6 +118,7 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_timit_labels_read", C.c_char_p, C.c_void_p, i64)
     sig("ks_cifar_read", C.c_char_p, C.c_void_p, C.c_void_p, i64, p_i64)
     sig("ks_last_fit_stats_json", i64, C.c_char_p, i64)
+    sig("ks_last_fit_stats_json_size", i64, p_i64)
     sig("ks_debug_gram", i64, i64, i64, C.c_void_p, i64, C.c_void_p, i64)
     sig("ks_debug_time_gram", i64, i64, i64, i32, p_f64)
     sig("ks_debug_chol_solve", i64, C.c_void_p, i32, C.c_void_p, i32, i32, C.c_void_p, p_f64)

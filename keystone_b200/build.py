@@ -15,8 +15,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libkeystone_b200.so")
-SOURCES = ["tc_kernels.cu", "aux_kernels.cu", "solve_kernels.cu", "engine.cu", "bwls.cu", "krr.cu", "io.cu"]
-HEADERS = ["tc_common.cuh", "kernels.h", "engine.h", os.path.join("..", "..", "include", "keystone_b200.h")]
+SOURCES = ["tc_kernels.cu", "aux_kernels.cu", "solve_kernels.cu", "engine.cu", "bwls.cu", "krr.cu", "lbfgs.cu", "io.cu"]
+HEADERS = ["tc_common.cuh", "kernels.h", "operand_split.cuh", "engine.h", os.path.join("..", "..", "include", "keystone_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "-DKS_BUILD",

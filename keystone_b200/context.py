@@ -90,8 +90,10 @@ class Context:
         return v.value
 
     def last_fit_stats(self) -> dict:
-        buf = C.create_string_buffer(4096)
-        check(self.handle, lib().ks_last_fit_stats_json(self.handle, buf, 4096))
+        n = C.c_int64(0)   # the JSON grows with the fit (DenseLBFGSwithL2 reports its loss history): size the buffer from it
+        check(self.handle, lib().ks_last_fit_stats_json_size(self.handle, C.byref(n)))
+        buf = C.create_string_buffer(max(int(n.value), 1))
+        check(self.handle, lib().ks_last_fit_stats_json(self.handle, buf, len(buf)))
         s = buf.value.decode()
         return json.loads(s) if s else {}
 

@@ -6,14 +6,9 @@
 #include <cuda_fp16.h>
 
 #include "kernels.h"
+#include "operand_split.cuh"
 
 namespace ks {
-
-__device__ __forceinline__ float round_tf32_aux(float x) {
-  uint32_t u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-  return __uint_as_float(u);
-}
 
 static inline unsigned grid_for(int64_t n, int threads, int64_t cap = 132 * 16) {
   int64_t g = (n + threads - 1) / threads;
@@ -214,8 +209,7 @@ __global__ void round_colsum_kernel(const float* __restrict__ R, float* __restri
         const int c = c4 + j;
         if (c < k) {
           a[j] += in[j];
-          o[j] = round_tf32_aux(in[j]);
-          l[j] = round_tf32_aux(in[j] - o[j]);  // split-operand mode: the tf32 rounding error, itself exact in fp32
+          tf32_pair(in[j], o[j], l[j]);  // l: the split-operand mode's lo plane
         } else {
           o[j] = 0.f;
           l[j] = 0.f;
@@ -262,8 +256,8 @@ __global__ void center_round_kernel(const float* __restrict__ F, int64_t ldf, in
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float v = (c4 + j < cols) ? F[r * ldf + c0 + c4 + j] - sh[j] : 0.f;  // c0 may be unaligned: scalar loads
-        o[j] = round_tf32_aux(v);
-        l[j] = slab_lo ? round_tf32_aux(v - o[j]) : 0.f;  // split-operand mode: hi + lo carries 21 bits of v
+        o[j] = round_tf32_rna(v);
+        l[j] = slab_lo ? round_tf32_rna(v - o[j]) : 0.f;  // split-operand mode: hi + lo carries 21 bits of v
         a[j] += o[j] + l[j];
       }
       *reinterpret_cast<float4*>(slab + r * lds + c4) = make_float4(o[0], o[1], o[2], o[3]);
@@ -418,8 +412,8 @@ __global__ void pack_update_kernel(const double* __restrict__ dW, double* __rest
       if (Wmodel) Wmodel[static_cast<int64_t>(c) * b + f] += w;
       if (delta) acc += delta[f] * w;
       const float wf = static_cast<float>(w);
-      h = round_tf32_aux(wf);
-      l = round_tf32_aux(static_cast<float>(w - static_cast<double>(h)));
+      h = round_tf32_rna(wf);
+      l = round_tf32_rna(static_cast<float>(w - static_cast<double>(h)));
     }
     bop_hi[static_cast<int64_t>(c) * ldb + f] = h;
     if (bop_lo) bop_lo[static_cast<int64_t>(c) * ldb + f] = l;
@@ -451,8 +445,8 @@ __global__ void pack_apply_kernel(const double* __restrict__ W, const double* __
     if (c < k && f < b) {
       const double w = W[static_cast<int64_t>(c) * b + f];
       if (mean) acc -= (mean[f] - static_cast<double>(shift32[f])) * w;
-      h = round_tf32_aux(static_cast<float>(w));
-      l = round_tf32_aux(static_cast<float>(w - static_cast<double>(h)));
+      h = round_tf32_rna(static_cast<float>(w));
+      l = round_tf32_rna(static_cast<float>(w - static_cast<double>(h)));
     }
     bop_hi[static_cast<int64_t>(c) * ldb + f] = h;
     if (bop_lo) bop_lo[static_cast<int64_t>(c) * ldb + f] = l;
@@ -479,7 +473,7 @@ __global__ void w_to_operand_kernel(const double* __restrict__ W, int64_t n_out,
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int64_t o = i / ld, c = i - o * ld;
     const float v = c < n_in ? static_cast<float>(W[c * n_out + o]) : 0.f;
-    dst[i] = round ? round_tf32_aux(v) : v;
+    dst[i] = round ? round_tf32_rna(v) : v;
   }
 }
 void launch_w_to_operand(const double* W_colmajor, int64_t n_out, int64_t n_in, float* dst, int64_t ld, cudaStream_t st, bool round) {
@@ -570,7 +564,7 @@ __global__ void fft_real_matrix_kernel(const double* __restrict__ signs, int64_t
       const int64_t q = (f * n) % P;                       // exact phase reduction in integers
       v = static_cast<float>((signs ? signs[n] : 1.0) * cospi(2.0 * static_cast<double>(q) / static_cast<double>(P)));
     }
-    dst[i] = round_tf32_aux(v);
+    dst[i] = round_tf32_rna(v);
     dst_full[i] = v;
   }
 }
@@ -744,14 +738,13 @@ __global__ void round_colsum16_kernel(const float* __restrict__ R, __half* __res
           o[j] = 0.f;
         }
       }
-      const __half2 h0 = __floats2half2_rn(o[0], o[1]), h1 = __floats2half2_rn(o[2], o[3]);
+      const __half2 h0 = f16_hi2(o[0], o[1]), h1 = f16_hi2(o[2], o[3]);
       uint2 pk;
       pk.x = *reinterpret_cast<const unsigned*>(&h0);
       pk.y = *reinterpret_cast<const unsigned*>(&h1);
       *reinterpret_cast<uint2*>(R16 + r * ld + c4) = pk;
       if (R16lo) {
-        const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-        const __half2 l0 = __floats2half2_rn(o[0] - f0.x, o[1] - f0.y), l1 = __floats2half2_rn(o[2] - f1.x, o[3] - f1.y);
+        const __half2 l0 = f16_lo2(o[0], o[1], h0), l1 = f16_lo2(o[2], o[3], h1);
         uint2 pl;
         pl.x = *reinterpret_cast<const unsigned*>(&l0);
         pl.y = *reinterpret_cast<const unsigned*>(&l1);

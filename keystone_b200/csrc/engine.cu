@@ -695,6 +695,10 @@ __global__ void scale_f64_to_f32_kernel(const double* src, double scale, float* 
   }
 }
 __global__ void set_f64_kernel(double* p, double v) { *p = v; }
+void launch_set_f64(double* p, double v, cudaStream_t st) { set_f64_kernel<<<1, 1, 0, st>>>(p, v); }
+void launch_scale_f64(const double* src, double scale, float* dst, double* dst64, int n, cudaStream_t st) {
+  if (n > 0) scale_f64_to_f32_kernel<<<(n + 255) / 256, 256, 0, st>>>(src, scale, dst, dst64, n);
+}
 __global__ void sumsq_f64_kernel(const double* p, int64_t n, double* out) {
   double acc = 0;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x)
@@ -1991,6 +1995,19 @@ KS_API int32_t ks_blockwls_fit(int64_t ctx, int64_t features, int64_t x_in, cons
   });
 }
 
+KS_API int32_t ks_lbfgs_fit(int64_t ctx, int64_t features, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int64_t labels,
+                            int32_t fit_intercept, int32_t num_corrections, double convergence_tol, int32_t num_iterations,
+                            double reg_param, int32_t precision_mode, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    const int prec = resolve_precision(c, precision_mode);
+    FeatSrc src;
+    make_feat_src(c, features, x_in, rfs, n_rfs, src, prec);
+    *out_model = fit_lbfgs(c, src, c.matrix(labels), fit_intercept != 0, num_corrections, convergence_tol, num_iterations, reg_param,
+                           prec);
+  });
+}
+
 KS_API int32_t ks_linear_map_fit(int64_t ctx, int64_t features, int64_t labels, int32_t has_lambda, double lambda, int64_t* out_model) {
   return guard(ctx, [&](Ctx& c) {
     if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
@@ -2343,6 +2360,12 @@ KS_API int32_t ks_kernel_model_from_host(int64_t ctx, int64_t kernel, const doub
   });
 }
 
+KS_API int32_t ks_last_fit_stats_json_size(int64_t ctx, int64_t* out_bytes) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_bytes) throw KsError{KS_ERR_INVALID, "null out_bytes"};
+    *out_bytes = static_cast<int64_t>(c.stats_json.size()) + 1;
+  });
+}
 KS_API int32_t ks_last_fit_stats_json(int64_t ctx, char* buf, int64_t buflen) {
   return guard(ctx, [&](Ctx& c) {
     if (!buf || buflen <= 0) throw KsError{KS_ERR_INVALID, "bad buffer"};

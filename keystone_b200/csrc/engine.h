@@ -314,6 +314,12 @@ void launch_update(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, c
 
 int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double lam, double w, int64_t nf_opt,
                  int precision = KS_PRECISION_TF32);
+// small device helpers (engine.cu): *p = v;  dst (fp32) / dst64 (fp64) [i] = src[i] * scale, either output may be null
+void launch_set_f64(double* p, double v, cudaStream_t st);
+void launch_scale_f64(const double* src, double scale, float* dst, double* dst64, int n, cudaStream_t st);
+// dense L-BFGS least squares (lbfgs.cu); collective
+int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int num_corrections, double convergence_tol, int num_iterations,
+                  double reg_param, int precision);
 // allocates the pinned mirror of a model whose brows / k / has_mean are set; enqueue_block_to_host copies block j (async, stream s)
 void model_alloc_host(Model& m);
 void model_block_to_host(Model& m, int j, cudaStream_t s);

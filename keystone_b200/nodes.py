@@ -12,6 +12,8 @@ Reference classes (K/ = src/main/scala/keystoneml/):
   BlockWeightedLeastSquaresEstimator  K/nodes/learning/BlockWeightedLeastSquares.scala:36-84
   BlockLinearMapper                   K/nodes/learning/BlockLinearMapper.scala:22-138
   LinearMapper / LinearMapEstimator   K/nodes/learning/LinearMapper.scala:18-116
+  DenseLBFGSwithL2                    K/nodes/learning/LBFGS.scala:135-192
+  LeastSquaresDenseGradient           K/nodes/learning/Gradient.scala:29-53
 
 Batches are ``DeviceMatrix`` / ``LazyFeatures`` (this rank's rows); 2-D numpy arrays are uploaded on
 the fly when a ``Context`` was given to the node.  No node computes on the host.
@@ -492,7 +494,9 @@ class BlockLinearMapper(Transformer):
         return out.value
 
 class LinearMapper(BlockLinearMapper):
-    """LinearMapper(x, bOpt, featureScaler): the single-block special case (LinearMapper.scala:18-63)."""
+    """LinearMapper(x, bOpt, featureScaler) (LinearMapper.scala:18-63): one weight matrix and one mean vector.  A model the
+    library stores in feature blocks (DenseLBFGSwithL2 streams its features block by block) is the same mapper: ``x`` and
+    ``feature_means`` join the blocks in feature order."""
 
     @classmethod
     def from_arrays(cls, ctx: Context, x: np.ndarray, b_opt=None, feature_mean=None):  # type: ignore[override]
@@ -501,7 +505,16 @@ class LinearMapper(BlockLinearMapper):
 
     @property
     def x(self) -> np.ndarray:
-        return self.xs[0]
+        xs = self.xs
+        return xs[0] if len(xs) == 1 else np.concatenate(xs, 0)
+
+    @property
+    def feature_means(self) -> Optional[List[np.ndarray]]:
+        """[mean] (one vector over all features), or None: StandardScalerModel's mean, as the reference's featureScaler."""
+        means = super().feature_means
+        if means is None or len(means) == 1:
+            return means
+        return [np.concatenate(means)]
 
 
 class BlockLeastSquaresEstimator(LabelEstimator, WeightedNode):
@@ -576,14 +589,80 @@ class LinearMapEstimator(LabelEstimator):
         return LinearMapper(ctx, h.value)
 
 
+class LeastSquaresDenseGradient:
+    """The least-squares gradient of dense L-BFGS (K/nodes/learning/Gradient.scala:29-53): (A W - Y) and A^T (A W - Y).  A marker:
+    the device computes it inside ``DenseLBFGSwithL2.fit``."""
+
+
+class DenseLBFGSwithL2(LabelEstimator, WeightedNode):
+    """``new DenseLBFGSwithL2(gradient, fitIntercept, numCorrections, convergenceTol, numIterations, regParam)``
+    (K/nodes/learning/LBFGS.scala:135-192) on the device: minimises |A_c W - Y_c|^2 / (2N) + regParam / 2 |W|^2 from W = 0.
+
+    Each step is the exact minimiser along the two-loop L-BFGS direction (the reference's Breeze line search is not
+    reproduced, DESIGN.md section 14), so the iterates differ from the reference's while the minimiser is the same.  The fit
+    stops after ``num_iterations`` steps or, with ``convergence_tol`` > 0, once max(last 10 losses) - f <= tol |f| or
+    max |g| <= max(tol |f|, 1e-8).  After a fit, ``loss_history`` holds f(W_0) .. f(W_T), ``iterations`` T and
+    ``stop_reason`` the rule that ended it.  ``precision`` as in ``BlockLeastSquaresEstimator``."""
+
+    def __init__(self, gradient=None, fit_intercept: bool = True, num_corrections: int = 10, convergence_tol: float = 1e-4,
+                 num_iterations: int = 100, reg_param: float = 0.0, ctx: Optional[Context] = None, precision: str = "default"):
+        gradient = LeastSquaresDenseGradient() if gradient is None else gradient
+        if not isinstance(gradient, LeastSquaresDenseGradient):
+            raise ValueError("DenseLBFGSwithL2 supports LeastSquaresDenseGradient only")
+        if int(num_corrections) < 1:
+            raise ValueError("num_corrections must be >= 1")
+        if int(num_iterations) < 1:
+            raise ValueError("num_iterations must be >= 1")
+        convergence_tol, reg_param = float(convergence_tol), float(reg_param)
+        if not (convergence_tol >= 0.0 and math.isfinite(convergence_tol)):
+            raise ValueError("convergence_tol must be finite and >= 0")
+        if not (reg_param >= 0.0 and math.isfinite(reg_param)):
+            raise ValueError("reg_param must be finite and >= 0")
+        if precision not in _capi.PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(_capi.PRECISIONS)}")
+        self.gradient, self.fit_intercept = gradient, bool(fit_intercept)
+        self.num_corrections, self.convergence_tol, self.num_iterations = int(num_corrections), convergence_tol, int(num_iterations)
+        self.reg_param, self.ctx, self.precision = reg_param, ctx, precision
+        self.weight = self.num_iterations + 1  # LBFGS.scala:144
+        self.loss_history: Optional[List[float]] = None
+        self.iterations: Optional[int] = None
+        self.stop_reason: Optional[str] = None
+        self.stats: Optional[dict] = None
+
+    def fit(self, data, labels) -> LinearMapper:
+        """Collective with several ranks (data and labels: this rank's rows)."""
+        ds = _as_dataset(self.ctx, data)
+        ctx = ds.ctx
+        lb = _as_dataset(ctx, labels)
+        f, x, rfs, n = feature_source_args(ds)
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_lbfgs_fit(ctx.handle, f, x, rfs, n, lb.handle, 1 if self.fit_intercept else 0, self.num_corrections,
+                                              self.convergence_tol, self.num_iterations, self.reg_param, _capi.PRECISIONS[self.precision],
+                                              C.byref(h)))
+        model = LinearMapper(ctx, h.value)
+        self.stats = ctx.last_fit_stats()
+        self.loss_history = [float(v) for v in self.stats["loss_history"]]
+        self.iterations, self.stop_reason = int(self.stats["iterations"]), self.stats["stop_reason"]
+        return model
+
+    def cost(self, n: int, d: int, k: int, sparsity: float, num_machines: int, cpu_weight: float, mem_weight: float,
+             network_weight: float) -> float:
+        """CostModel.cost (LBFGS.scala:175-191)."""
+        flops = float(n) * d * k / num_machines
+        bytes_scanned = float(n) * d / num_machines
+        network = 2.0 * d * k * math.log(num_machines) / math.log(2.0)
+        return self.num_iterations * (max(cpu_weight * flops, mem_weight * bytes_scanned) + network_weight * network)
+
+
 class LeastSquaresEstimator(LabelEstimator, WeightedNode):
     """The reference's cost-model-driven solver choice (K/nodes/learning/LeastSquaresEstimator.scala:17-87): the four
     options' ``CostModel.cost`` formulas -- dense L-BFGS (K/nodes/learning/LBFGS.scala:175-191), sparse L-BFGS (:264-280),
     ``BlockLeastSquaresEstimator(1000, 3, lambda)`` (BlockLinearMapper.scala:268-282) and ``LinearMapEstimator(Some(lambda))``
     (LinearMapper.scala:100-115) -- with the reference's empirical weights; ``optimize`` returns the cheapest.
 
-    On this engine the two direct solvers run on the GPU.  The L-BFGS options are not part of the hot path (SURVEY 2.1): when
-    the cost model prefers one of them, ``fit`` runs the GPU block solver instead and records both in ``selected`` / ``used``."""
+    ``fit`` runs the two direct solvers on the GPU.  When the cost model prefers an L-BFGS option, ``fit`` runs the GPU block
+    solver instead and records both in ``selected`` / ``used``.  ``DenseLBFGSwithL2`` exists on the device too, but this routing
+    is kept until measurements say where it beats the block solver (DESIGN.md section 14)."""
 
     def __init__(self, lam: float = 0.0, num_machines: Optional[int] = None, cpu_weight: float = 3.8e-4, mem_weight: float = 2.9e-1,
                  network_weight: float = 1.32, ctx: Optional[Context] = None):
@@ -594,12 +673,12 @@ class LeastSquaresEstimator(LabelEstimator, WeightedNode):
         self.used: Optional[str] = None
 
     @staticmethod
-    def _lbfgs_cost(n, d, k, sparsity, m, cw, mw, nw, sparse: bool, num_iterations: int = 20, sparse_overhead: float = 8.0):
-        dens = sparsity if sparse else 1.0
-        flops = float(n) * dens * d * k / m
-        bytes_scanned = float(n) * d * dens / m
+    def _sparse_lbfgs_cost(n, d, k, sparsity, m, cw, mw, nw, num_iterations: int = 20, sparse_overhead: float = 8.0):
+        """SparseLBFGSwithL2.cost (LBFGS.scala:264-280)."""
+        flops = float(n) * sparsity * d * k / m
+        bytes_scanned = float(n) * d * sparsity / m
         network = 2.0 * d * k * math.log(m) / math.log(2.0)
-        return num_iterations * ((sparse_overhead if sparse else 1.0) * max(cw * flops, mw * bytes_scanned) + nw * network)
+        return num_iterations * (sparse_overhead * max(cw * flops, mw * bytes_scanned) + nw * network)
 
     def costs(self, n: int, d: int, k: int, sparsity: float, num_machines: int) -> dict:
         cw, mw, nw = self.cpu_weight, self.mem_weight, self.network_weight
@@ -607,8 +686,8 @@ class LeastSquaresEstimator(LabelEstimator, WeightedNode):
         exact_flops = float(n) * d * (d + k) / num_machines
         exact_bytes = float(n) * d / num_machines + float(d) * d
         return {
-            "dense_lbfgs": self._lbfgs_cost(n, d, k, sparsity, num_machines, cw, mw, nw, False),
-            "sparse_lbfgs": self._lbfgs_cost(n, d, k, sparsity, num_machines, cw, mw, nw, True),
+            "dense_lbfgs": DenseLBFGSwithL2(num_iterations=20).cost(n, d, k, sparsity, num_machines, cw, mw, nw),
+            "sparse_lbfgs": self._sparse_lbfgs_cost(n, d, k, sparsity, num_machines, cw, mw, nw),
             "block": block.cost(n, d, k, sparsity, num_machines, cw, mw, nw),
             "exact": max(cw * exact_flops, mw * exact_bytes) + nw * float(d) * (d + k),
         }

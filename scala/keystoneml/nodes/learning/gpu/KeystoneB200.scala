@@ -32,6 +32,8 @@ class KeystoneB200 extends Serializable {
   @native def blockWlsFit(ctx: Long, features: Long, xIn: Long, rfs: Array[Long], labels: Long,
       blockSize: Int, numIter: Int, lambda: Double, mixtureWeight: Double, numFeaturesOr0: Long, precisionMode: Int): Long
   @native def linearMapFit(ctx: Long, features: Long, labels: Long, hasLambda: Boolean, lambda: Double): Long
+  @native def lbfgsFit(ctx: Long, features: Long, xIn: Long, rfs: Array[Long], labels: Long, fitIntercept: Boolean,
+      numCorrections: Int, convergenceTol: Double, numIterations: Int, regParam: Double, precisionMode: Int): Long
 
   @native def modelFromHost(ctx: Long, xs: Array[Array[Double]], blockSize: Int, k: Long, b: Array[Double],
       means: Array[Array[Double]]): Long
