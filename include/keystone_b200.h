@@ -179,6 +179,27 @@ KS_API int32_t ks_lbfgs_fit(int64_t ctx, int64_t features, int64_t x_in, const i
                             int32_t fit_intercept, int32_t num_corrections, double convergence_tol, int32_t num_iterations,
                             double reg_param, int32_t precision_mode, int64_t* out_model);
 
+/* ---- covariance-based transforms (DESIGN.md section 15) -------------------------------------
+ * Every product of these fits runs in fp64 on the DMMA tensor core; they take no precision mode.  The fitted objects are ordinary
+ * model handles (apply, save / load, host views): apply runs in the context's precision like every model.  x: this rank's rows
+ * (any rank may hold fewer than d rows, or none).  Rank 0's eigen / SVD / CholeskyQR factors are broadcast, so the models are
+ * bit-identical across ranks.  All are collective. */
+/* PCAEstimator(dims) / DistributedPCAEstimator(dims).fit (K/nodes/learning/PCA.scala:157-199, DistributedPCA.scala:30-56): eigenvectors
+ * of the exactly centred covariance, descending, MATLAB sign convention, the first dims -> model (d x dims, no mean, no intercept:
+ * PCATransformer does not centre).  dims in [1, d]. */
+KS_API int32_t ks_pca_fit(int64_t ctx, int64_t x, int32_t dims, int64_t* out_model);
+/* ZCAWhitenerEstimator(eps).fitSingle (K/nodes/learning/ZCAWhitener.scala:37-72) -> model (d x d whitener V diag(w) V^T with
+ * w = (lambda / (N - 1) + eps)^-1/2, feature means = column means).  Needs N >= d rows over all ranks; eps finite and >= 0. */
+KS_API int32_t ks_zca_fit(int64_t ctx, int64_t x, double eps, int64_t* out_model);
+/* ApproximatePCAEstimator.approximateQ (K/nodes/learning/ApproximatePCA.scala:69-85): this rank's rows of the orthonormal N x l
+ * basis, as an fp32 matrix.  omega: the caller's d x l Gaussian test matrix (column-major); l in [1, min(N, d)], q >= 0.  The QR of
+ * every tall-skinny factor is shifted CholeskyQR3. */
+KS_API int32_t ks_approx_range(int64_t ctx, int64_t x, const double* omega_colmajor /* d x l */, int32_t l, int32_t q, int64_t* out_q);
+/* ApproximatePCAEstimator(dims, q, p).fit (ApproximatePCA.scala:37-58) with the caller's omega (d x (dims + p), column-major) ->
+ * model (d x dims, no mean, no intercept).  No centring, like the reference. */
+KS_API int32_t ks_approx_pca_fit(int64_t ctx, int64_t x, const double* omega_colmajor, int32_t dims, int32_t q, int32_t p,
+                                 int64_t* out_model);
+
 /* ---- BlockLinearMapper / LinearMapper state (K/nodes/learning/BlockLinearMapper.scala:22-33,
  * K/nodes/learning/LinearMapper.scala:18-22) ------------------------------------------------ */
 KS_API int32_t ks_model_from_host(int64_t ctx, const double* const* xs_colmajor, const int64_t* block_rows, int32_t n_blocks,
@@ -273,6 +294,10 @@ KS_API int32_t ks_ctx_launch_count(int64_t ctx, int64_t* out_count);
 KS_API int32_t ks_debug_gram(int64_t ctx, int64_t a, int64_t b, double* out_g, int64_t ld_g, double* out_c, int64_t ld_c);
 /* Times `iters` launches of the Gram kernel alone (CUDA events on the launching stream); returns ms per launch. */
 KS_API int32_t ks_debug_time_gram(int64_t ctx, int64_t a, int64_t b, int32_t iters, double* out_ms);
+/* out (m x n, row-major fp64, ld_out) = (A - 1 s^T)^T (B - 1 t^T) through the fp64 DMMA Gram of the PCA fits; b = 0: symmetric mode
+ * (B = A, t = s); either shift may be NULL (zero).  Not collective. */
+KS_API int32_t ks_debug_gram_f64(int64_t ctx, int64_t a, int64_t b_or_0, const double* shift_a_or_null, const double* shift_b_or_null,
+                                 double* out, int64_t ld_out);
 
 /* X = H^-1 B for a symmetric positive definite H (column-major n x n) and B (column-major n x k): Cholesky with cuSOLVER, then
  * either the library's own multi-RHS solve kernel (use_cusolver = 0; option "custom_solve") or cusolverDnDpotrs (the default of

@@ -162,6 +162,31 @@ JFN(jlong, linearMapFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong 
   return ok(env, ctx, ks_linear_map_fit(ctx, features, labels, hasLambda ? 1 : 0, lambda, &h)) ? h : 0;
 }
 
+// ---- PCA / ZCA whitening / approximate PCA (models are ordinary model handles)
+JFN(jlong, pcaFit)(JNIEnv* env, jobject, jlong ctx, jlong x, jint dims) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_pca_fit(ctx, x, dims, &h)) ? h : 0;
+}
+JFN(jlong, zcaFit)(JNIEnv* env, jobject, jlong ctx, jlong x, jdouble eps) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_zca_fit(ctx, x, eps, &h)) ? h : 0;
+}
+// omega: the d x l test matrix as DenseMatrix.data (column-major)
+JFN(jlong, approxRange)(JNIEnv* env, jobject, jlong ctx, jlong x, jdoubleArray omega, jint l, jint q) {
+  int64_t h = 0;
+  jdouble* om = omega ? env->GetDoubleArrayElements(omega, nullptr) : nullptr;
+  const int32_t rc = ks_approx_range(ctx, x, om, l, q, &h);
+  if (om) env->ReleaseDoubleArrayElements(omega, om, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, approxPcaFit)(JNIEnv* env, jobject, jlong ctx, jlong x, jdoubleArray omega, jint dims, jint q, jint p) {
+  int64_t h = 0;
+  jdouble* om = omega ? env->GetDoubleArrayElements(omega, nullptr) : nullptr;
+  const int32_t rc = ks_approx_pca_fit(ctx, x, om, dims, q, p, &h);
+  if (om) env->ReleaseDoubleArrayElements(omega, om, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+
 // ---- models
 JFN(jlong, modelFromHost)(JNIEnv* env, jobject, jlong ctx, jobjectArray xs, jint blockSize, jlong k, jdoubleArray bOrNull,
                           jobjectArray meansOrNull) {

@@ -7,6 +7,16 @@ from ._capi import KeystoneError, LIB_PATH, declared_symbols  # noqa: F401
 from .context import Context, DeviceMatrix, LazyFeatures, shard_range  # noqa: F401
 from .workflow import Estimator, LabelEstimator, Pipeline, Transformer  # noqa: F401
 from .nodes import (  # noqa: F401
+    ApproximatePCAEstimator,
+    BatchPCATransformer,
+    ColumnPCAEstimator,
+    DistributedColumnPCAEstimator,
+    DistributedPCAEstimator,
+    LocalColumnPCAEstimator,
+    PCAEstimator,
+    PCATransformer,
+    ZCAWhitener,
+    ZCAWhitenerEstimator,
     BlockLeastSquaresEstimator,
     BlockLinearMapper,
     BlockWeightedLeastSquaresEstimator,

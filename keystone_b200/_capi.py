@@ -91,6 +91,11 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_blockwls_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, f64, i64, i32, p_i64)
     sig("ks_linear_map_fit", i64, i64, i64, i32, f64, p_i64)
     sig("ks_lbfgs_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, i32, f64, i32, p_i64)
+    sig("ks_pca_fit", i64, i64, i32, p_i64)
+    sig("ks_zca_fit", i64, i64, f64, p_i64)
+    sig("ks_approx_range", i64, i64, C.c_void_p, i32, i32, p_i64)
+    sig("ks_approx_pca_fit", i64, i64, C.c_void_p, i32, i32, i32, p_i64)
+    sig("ks_debug_gram_f64", i64, i64, i64, C.c_void_p, C.c_void_p, C.c_void_p, i64)
     sig("ks_model_from_host", i64, pp_f64, p_i64, i32, i64, C.c_void_p, pp_f64, i32, p_i64)
     sig("ks_model_num_blocks", i64, i64, p_i32, p_i64, p_i32)
     sig("ks_model_block_rows", i64, i64, i32, p_i64)

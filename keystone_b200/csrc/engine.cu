@@ -45,6 +45,12 @@ SolverApi& solver_api() {
       load_sym(api.lib, "cusolverDnDpotrf_bufferSize", api.DpotrfBufferSize, "libcusolver");
       load_sym(api.lib, "cusolverDnDpotrf", api.Dpotrf, "libcusolver");
       load_sym(api.lib, "cusolverDnDpotrs", api.Dpotrs, "libcusolver");
+      load_sym(api.lib, "cusolverDnDsyevd_bufferSize", api.DsyevdBufferSize, "libcusolver");
+      load_sym(api.lib, "cusolverDnDsyevd", api.Dsyevd, "libcusolver");
+      load_sym(api.lib, "cusolverDnDgesvd_bufferSize", api.DgesvdBufferSize, "libcusolver");
+      load_sym(api.lib, "cusolverDnDgesvd", api.Dgesvd, "libcusolver");
+      load_sym(api.lib, "cusolverDnXtrtri_bufferSize", api.XtrtriBufferSize, "libcusolver");
+      load_sym(api.lib, "cusolverDnXtrtri", api.Xtrtri, "libcusolver");
     } catch (const KsError& e) {
       fail = e.msg;
     }
@@ -2016,6 +2022,39 @@ KS_API int32_t ks_linear_map_fit(int64_t ctx, int64_t features, int64_t labels, 
     // one block spanning every feature, one pass: exactly (A^T A [+ lambda I]) \ A^T y on centred data; the operand mode is the
     // context's ("precision" option; the default is the split-operand parity mode)
     *out_model = fit_blockls(c, src, c.matrix(labels), static_cast<int>(src.D), 1, has_lambda ? lambda : 0.0, 0, c.precision);
+  });
+}
+
+// ---------------------------------------------------------------- covariance-based transforms (pca.cu)
+KS_API int32_t ks_pca_fit(int64_t ctx, int64_t x, int32_t dims, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    *out_model = fit_pca(c, c.matrix(x), dims);
+  });
+}
+KS_API int32_t ks_zca_fit(int64_t ctx, int64_t x, double eps, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    *out_model = fit_zca(c, c.matrix(x), eps);
+  });
+}
+KS_API int32_t ks_approx_range(int64_t ctx, int64_t x, const double* omega_colmajor, int32_t l, int32_t q, int64_t* out_q) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_q) throw KsError{KS_ERR_INVALID, "null out_q"};
+    *out_q = approx_range(c, c.matrix(x), omega_colmajor, l, q);
+  });
+}
+KS_API int32_t ks_approx_pca_fit(int64_t ctx, int64_t x, const double* omega_colmajor, int32_t dims, int32_t q, int32_t p,
+                                 int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    *out_model = fit_approx_pca(c, c.matrix(x), omega_colmajor, dims, q, p);
+  });
+}
+KS_API int32_t ks_debug_gram_f64(int64_t ctx, int64_t a, int64_t b_or_0, const double* shift_a_or_null, const double* shift_b_or_null,
+                                 double* out, int64_t ld_out) {
+  return guard(ctx, [&](Ctx& c) {
+    debug_gram_f64(c, c.matrix(a), b_or_0 ? &c.matrix(b_or_0) : nullptr, shift_a_or_null, shift_b_or_null, out, ld_out);
   });
 }
 

@@ -148,6 +148,17 @@ struct SolverApi {
   cusolverStatus_t (*DpotrfBufferSize)(cusolverDnHandle_t, cublasFillMode_t, int, double*, int, int*) = nullptr;
   cusolverStatus_t (*Dpotrf)(cusolverDnHandle_t, cublasFillMode_t, int, double*, int, double*, int, int*) = nullptr;
   cusolverStatus_t (*Dpotrs)(cusolverDnHandle_t, cublasFillMode_t, int, int, const double*, int, double*, int, int*) = nullptr;
+  // PCA / ZCA / ApproximatePCA (pca.cu)
+  cusolverStatus_t (*DsyevdBufferSize)(cusolverDnHandle_t, cusolverEigMode_t, cublasFillMode_t, int, const double*, int, const double*,
+                                       int*) = nullptr;
+  cusolverStatus_t (*Dsyevd)(cusolverDnHandle_t, cusolverEigMode_t, cublasFillMode_t, int, double*, int, double*, double*, int, int*) = nullptr;
+  cusolverStatus_t (*DgesvdBufferSize)(cusolverDnHandle_t, int, int, int*) = nullptr;
+  cusolverStatus_t (*Dgesvd)(cusolverDnHandle_t, signed char, signed char, int, int, double*, int, double*, double*, int, double*, int,
+                             double*, int, double*, int*) = nullptr;
+  cusolverStatus_t (*XtrtriBufferSize)(cusolverDnHandle_t, cublasFillMode_t, cublasDiagType_t, int64_t, cudaDataType, void*, int64_t,
+                                       size_t*, size_t*) = nullptr;
+  cusolverStatus_t (*Xtrtri)(cusolverDnHandle_t, cublasFillMode_t, cublasDiagType_t, int64_t, cudaDataType, void*, int64_t, void*, size_t,
+                             void*, size_t, int*) = nullptr;
 };
 struct NcclApi {
   void* lib = nullptr;
@@ -334,5 +345,13 @@ int64_t fit_krr(Ctx& c, const std::shared_ptr<GaussKernel>& K, Matrix& Y, double
 std::unique_ptr<Matrix> kernel_model_apply(Ctx& c, Model& md, Matrix& x);
 int64_t kernel_model_from_host(Ctx& c, const std::shared_ptr<GaussKernel>& K, const double* const* xs, const int64_t* block_rows,
                                int32_t n_blocks, int64_t k, int32_t block_size);
+
+// PCA, ZCA whitening and approximate PCA on the fp64 DMMA kernels (pca.cu); all collective
+int64_t fit_pca(Ctx& c, Matrix& X, int dims);
+int64_t fit_zca(Ctx& c, Matrix& X, double eps);
+int64_t approx_range(Ctx& c, Matrix& X, const double* omega_colmajor, int l, int q);  // returns a matrix handle
+int64_t fit_approx_pca(Ctx& c, Matrix& X, const double* omega_colmajor, int dims, int q, int p);
+// out (m x n, row-major fp64, host) = (A - 1 s^T)^T (B - 1 t^T); B null: symmetric mode.  Not collective.
+void debug_gram_f64(Ctx& c, Matrix& A, Matrix* B, const double* shift_a, const double* shift_b, double* out, int64_t ld_out);
 
 }  // namespace ks

@@ -867,6 +867,244 @@ class KernelRidgeRegression(LabelEstimator):
         return KernelBlockLinearMapper(ctx, h.value, transformer)
 
 
+# ------------------------------------------------------------------------------------------ PCA and ZCA whitening
+class PCATransformer(LinearMapper):
+    """``new PCATransformer(pcaMat)`` (K/nodes/learning/PCA.scala:19-31): x -> pcaMat^T x, a LinearMapper with no mean and no
+    intercept (the reference does not centre).  ``pca_mat`` is d x dims."""
+
+    @property
+    def pca_mat(self) -> np.ndarray:
+        return self.x
+
+    @classmethod
+    def from_matrix(cls, ctx: Context, pca_mat: np.ndarray) -> "PCATransformer":
+        return cls.from_arrays(ctx, np.asarray(pca_mat, dtype=np.float64))
+
+
+class BatchPCATransformer(Transformer):
+    """``BatchPCATransformer(pcaMat)`` (PCA.scala:39-44): each (d x m_i) item -> pcaMat^T M_i (dims x m_i).  The columns of all items
+    go through one device apply."""
+
+    def __init__(self, transformer: PCATransformer):
+        self.transformer = transformer
+
+    @property
+    def pca_mat(self) -> np.ndarray:
+        return self.transformer.pca_mat
+
+    def apply(self, data):
+        single = isinstance(data, np.ndarray) and data.ndim == 2
+        items = [np.asarray(data)] if single else [np.asarray(m) for m in data]
+        d = self.pca_mat.shape[0]
+        for m in items:
+            if m.ndim != 2 or m.shape[0] != d:
+                raise ValueError(f"every item must have {d} rows")
+        rows = np.concatenate([m.T for m in items], 0).astype(np.float32)
+        out = self.transformer.apply(self.transformer.ctx.matrix(rows)).to_numpy()
+        offs = np.cumsum([0] + [m.shape[1] for m in items])
+        res = [np.ascontiguousarray(out[offs[i]:offs[i + 1]].T) for i in range(len(items))]
+        return res[0] if single else res
+
+
+def _device_matrix(ctx: Optional[Context], data) -> DeviceMatrix:
+    """A materialised device matrix of ``data`` (lazy feature sources are materialised first, as LinearMapEstimator.fit does)."""
+    ds = _as_dataset(ctx, data)
+    return ds if isinstance(ds, DeviceMatrix) else ds.materialize()
+
+
+def _check_dims(dims) -> int:
+    if int(dims) < 1:
+        raise ValueError("dims must be >= 1")
+    return int(dims)
+
+
+class PCAEstimator(Estimator):
+    """``new PCAEstimator(dims)`` (PCA.scala:157-225): the first ``dims`` eigenvectors of the exactly centred covariance, in
+    descending order with the MATLAB sign convention.  The covariance is an fp64 DMMA Gram over the row shards and the eigenproblem
+    is solved in fp64 (DESIGN.md section 15); after a fit ``eigenvalues`` holds the leading dims eigenvalues of X_c^T X_c."""
+
+    def __init__(self, dims: int, ctx: Optional[Context] = None):
+        self.dims, self.ctx = _check_dims(dims), ctx
+        self.stats: Optional[dict] = None
+        self.eigenvalues: Optional[np.ndarray] = None
+
+    def fit(self, data) -> PCATransformer:
+        """Collective with several ranks (data: this rank's rows)."""
+        x = _device_matrix(self.ctx, data)
+        h = C.c_int64(0)
+        check(x.ctx.handle, lib().ks_pca_fit(x.ctx.handle, x.handle, self.dims, C.byref(h)))
+        model = PCATransformer(x.ctx, h.value)
+        self.stats = x.ctx.last_fit_stats()
+        self.eigenvalues = np.asarray(self.stats["eigenvalues"], dtype=np.float64)
+        return model
+
+    def cost(self, n: int, d: int, k: int, sparsity: float, num_machines: int, cpu_weight: float, mem_weight: float,
+             network_weight: float) -> float:
+        """CostModel.cost (PCA.scala:211-224)."""
+        flops = float(n) * d * d
+        bytes_scanned = float(n) * d
+        network = float(n) * d
+        return max(cpu_weight * flops, mem_weight * bytes_scanned) + network_weight * network
+
+
+class DistributedPCAEstimator(PCAEstimator):
+    """``new DistributedPCAEstimator(dims)`` (K/nodes/learning/DistributedPCA.scala:20-74).  The reference's TSQR-then-SVD and the
+    local SVD give the same components; on the device both are one algorithm, because the rows are sharded already."""
+
+    def cost(self, n: int, d: int, k: int, sparsity: float, num_machines: int, cpu_weight: float, mem_weight: float,
+             network_weight: float) -> float:
+        """CostModel.cost (DistributedPCA.scala:59-73)."""
+        log2m = math.log(num_machines) / math.log(2.0)
+        flops = float(n) * d * d / num_machines + float(d) * d * d * log2m
+        bytes_scanned = float(n) * d
+        network = float(d) * d * log2m
+        return max(cpu_weight * flops, mem_weight * bytes_scanned) + network_weight * network
+
+
+def _columns_as_rows(data) -> np.ndarray:
+    """The columns of every (d x m_i) item as rows (MatrixUtils.matrixToColArray)."""
+    items = [np.asarray(data)] if isinstance(data, np.ndarray) and data.ndim == 2 else [np.asarray(m) for m in data]
+    return np.concatenate([m.T for m in items], 0).astype(np.float32)
+
+
+class LocalColumnPCAEstimator(Estimator):
+    """``LocalColumnPCAEstimator(dims)`` (PCA.scala:51-72): PCA over the columns of (d x m_i) items -> BatchPCATransformer."""
+
+    _inner = PCAEstimator
+
+    def __init__(self, dims: int, ctx: Optional[Context] = None):
+        self.dims, self.ctx = _check_dims(dims), ctx
+        self.pca_estimator = self._inner(dims, ctx)
+
+    def fit(self, data) -> BatchPCATransformer:
+        if self.ctx is None:
+            raise KeystoneError(-1, "numpy input needs a Context (pass ctx= to the node)")
+        return BatchPCATransformer(self.pca_estimator.fit(self.ctx.matrix(_columns_as_rows(data))))
+
+    def cost(self, n, d, k, sparsity, num_machines, cpu_weight, mem_weight, network_weight) -> float:
+        return self.pca_estimator.cost(n, d, k, sparsity, num_machines, cpu_weight, mem_weight, network_weight)
+
+
+class DistributedColumnPCAEstimator(LocalColumnPCAEstimator):
+    """``DistributedColumnPCAEstimator(dims)`` (PCA.scala:81-102)."""
+
+    _inner = DistributedPCAEstimator
+
+
+class ColumnPCAEstimator(Estimator):
+    """``ColumnPCAEstimator(dims, numMachines, cpuWeight, memWeight, networkWeight)`` (PCA.scala:117-151): ``optimize`` picks the
+    local or the distributed column estimator by their costs (host-only arithmetic); ``fit`` uses the distributed one, the
+    reference's default."""
+
+    def __init__(self, dims: int, num_machines: Optional[int] = None, cpu_weight: float = 3.8e-4, mem_weight: float = 2.9e-1,
+                 network_weight: float = 1.32, ctx: Optional[Context] = None):
+        self.dims, self.num_machines, self.ctx = _check_dims(dims), num_machines, ctx
+        self.cpu_weight, self.mem_weight, self.network_weight = cpu_weight, mem_weight, network_weight
+        self.local_estimator = LocalColumnPCAEstimator(dims, ctx)
+        self.distributed_estimator = DistributedColumnPCAEstimator(dims, ctx)
+        self.default = self.distributed_estimator
+
+    def optimize(self, sample: Sequence[np.ndarray], num_per_partition: dict) -> LocalColumnPCAEstimator:
+        """sample: (d x m_i) items; num_per_partition: items per partition of the full dataset (WorkflowUtils.numPerPartition)."""
+        cols_per_matrix = sum(np.asarray(m).shape[1] for m in sample) / float(len(sample))
+        n = int(cols_per_matrix * sum(num_per_partition.values()))
+        d = np.asarray(sample[0]).shape[0]
+        m = self.num_machines or 1
+        args = (n, d, self.dims, 1.0, m, self.cpu_weight, self.mem_weight, self.network_weight)
+        local, dist = self.local_estimator.cost(*args), self.distributed_estimator.cost(*args)
+        return self.local_estimator if local < dist else self.distributed_estimator
+
+    def fit(self, data) -> BatchPCATransformer:
+        return self.default.fit(data)
+
+
+class ApproximatePCAEstimator(Estimator):
+    """``new ApproximatePCAEstimator(dims, q, p)`` (K/nodes/learning/ApproximatePCA.scala:21-58; Halko, Martinsson and Tropp 2011,
+    Algorithms 4.4 and 5.1) on the raw, uncentred data.  The Gaussian test matrix Omega (d x (dims + p)) is drawn on the host by
+    ``ApproximatePCAEstimator.omega``: ``numpy.random.default_rng(seed).standard_normal``.  Breeze's MersenneTwister stream is not
+    reproduced.  The QR of every tall-skinny factor is shifted CholeskyQR3 in fp64 (DESIGN.md section 15)."""
+
+    def __init__(self, dims: int, q: int = 10, p: int = 5, seed: int = 0, ctx: Optional[Context] = None):
+        if int(q) < 0:
+            raise ValueError("q must be >= 0")
+        if int(p) < 0:
+            raise ValueError("p must be >= 0")
+        self.dims, self.q, self.p, self.seed, self.ctx = _check_dims(dims), int(q), int(p), seed, ctx
+        self.stats: Optional[dict] = None
+        self.singular_values: Optional[np.ndarray] = None
+
+    @staticmethod
+    def omega(d: int, l: int, seed: int = 0) -> np.ndarray:
+        """The d x l Gaussian test matrix of a fit with this seed."""
+        return np.random.default_rng(seed).standard_normal((int(d), int(l)))
+
+    def fit(self, data) -> PCATransformer:
+        """Collective with several ranks (data: this rank's rows; every rank draws the same Omega)."""
+        x = _device_matrix(self.ctx, data)
+        om = np.asfortranarray(self.omega(x.cols, self.dims + self.p, self.seed))
+        h = C.c_int64(0)
+        check(x.ctx.handle, lib().ks_approx_pca_fit(x.ctx.handle, x.handle, om.ctypes.data_as(C.c_void_p), self.dims, self.q, self.p,
+                                                     C.byref(h)))
+        model = PCATransformer(x.ctx, h.value)
+        self.stats = x.ctx.last_fit_stats()
+        self.singular_values = np.asarray(self.stats["singular_values"], dtype=np.float64)
+        return model
+
+    @staticmethod
+    def approximate_q(data, l: int, q: int, seed: int = 0, ctx: Optional[Context] = None) -> DeviceMatrix:
+        """``ApproximatePCAEstimator.approximateQ(A, l, q, seed)`` (ApproximatePCA.scala:69-85): this rank's rows of the orthonormal
+        N x l basis, as an fp32 device matrix."""
+        x = _device_matrix(ctx, data)
+        om = np.asfortranarray(ApproximatePCAEstimator.omega(x.cols, l, seed))
+        h = C.c_int64(0)
+        check(x.ctx.handle, lib().ks_approx_range(x.ctx.handle, x.handle, om.ctypes.data_as(C.c_void_p), int(l), int(q), C.byref(h)))
+        return DeviceMatrix(x.ctx, h.value, x.rows, int(l))
+
+
+class ZCAWhitener(LinearMapper):
+    """``new ZCAWhitener(whitener, means)`` (K/nodes/learning/ZCAWhitener.scala:12-19): (in - means) * whitener, a LinearMapper
+    with the means as its feature scaler."""
+
+    @property
+    def whitener(self) -> np.ndarray:
+        return self.x
+
+    @property
+    def means(self) -> np.ndarray:
+        return self.feature_means[0]
+
+    @classmethod
+    def from_whitener(cls, ctx: Context, whitener: np.ndarray, means: np.ndarray) -> "ZCAWhitener":
+        return cls.from_arrays(ctx, np.asarray(whitener, dtype=np.float64), None, np.asarray(means, dtype=np.float64))
+
+
+class ZCAWhitenerEstimator(Estimator):
+    """``new ZCAWhitenerEstimator(eps)`` (ZCAWhitener.scala:30-72): whitener = V diag((lambda / (N - 1) + eps)^-1/2) V^T from the
+    eigenpairs of the exactly centred covariance, all in fp64 on the device (DESIGN.md section 15).  Needs at least d rows."""
+
+    def __init__(self, eps: float = 0.1, ctx: Optional[Context] = None):
+        eps = float(eps)
+        if not (eps >= 0.0 and math.isfinite(eps)):
+            raise ValueError("eps must be finite and >= 0")
+        self.eps, self.ctx = eps, ctx
+        self.stats: Optional[dict] = None
+
+    def fit_single(self, matrix) -> ZCAWhitener:
+        """Collective with several ranks (matrix: this rank's rows)."""
+        x = _device_matrix(self.ctx, matrix)
+        h = C.c_int64(0)
+        check(x.ctx.handle, lib().ks_zca_fit(x.ctx.handle, x.handle, self.eps, C.byref(h)))
+        model = ZCAWhitener(x.ctx, h.value)
+        self.stats = x.ctx.last_fit_stats()
+        return model
+
+    def fit(self, data) -> ZCAWhitener:
+        """Fits on the first item of a sequence of matrices (ZCAWhitener.scala:33-35); a single matrix is its own first item."""
+        if isinstance(data, (list, tuple)):
+            data = data[0]
+        return self.fit_single(data)
+
+
 class StandardScalerModel(Transformer):
     """(x - mean) [/ std] as a LinearMapper-free node is out of the hot path; the fits above centre internally
     (BlockLinearMapper.scala:224-232).  Kept for API parity: holds the statistics a fitted model reports."""

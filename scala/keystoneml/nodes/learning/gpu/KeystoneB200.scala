@@ -34,6 +34,11 @@ class KeystoneB200 extends Serializable {
   @native def linearMapFit(ctx: Long, features: Long, labels: Long, hasLambda: Boolean, lambda: Double): Long
   @native def lbfgsFit(ctx: Long, features: Long, xIn: Long, rfs: Array[Long], labels: Long, fitIntercept: Boolean,
       numCorrections: Int, convergenceTol: Double, numIterations: Int, regParam: Double, precisionMode: Int): Long
+  /** PCA / ZCA / approximate PCA (collective, fp64 on the device); omega is the d x l test matrix, DenseMatrix.data. */
+  @native def pcaFit(ctx: Long, x: Long, dims: Int): Long
+  @native def zcaFit(ctx: Long, x: Long, eps: Double): Long
+  @native def approxRange(ctx: Long, x: Long, omega: Array[Double], l: Int, q: Int): Long
+  @native def approxPcaFit(ctx: Long, x: Long, omega: Array[Double], dims: Int, q: Int, p: Int): Long
 
   @native def modelFromHost(ctx: Long, xs: Array[Array[Double]], blockSize: Int, k: Long, b: Array[Double],
       means: Array[Array[Double]]): Long
