@@ -298,6 +298,25 @@ KS_API int32_t ks_debug_time_gram(int64_t ctx, int64_t a, int64_t b, int32_t ite
  * (B = A, t = s); either shift may be NULL (zero).  Not collective. */
 KS_API int32_t ks_debug_gram_f64(int64_t ctx, int64_t a, int64_t b_or_0, const double* shift_a_or_null, const double* shift_b_or_null,
                                  double* out, int64_t ld_out);
+/* The projection GEMM of generated features alone: feature columns [c0, c0 + cols) of rows [row_begin, row_begin + rows) of
+ * x_in + rfs[n_rfs] (cosine or PaddedFFT maps), minus shift_or_null (cols values; NULL: zero), produced by the same feature
+ * source and launch as in the fits.  The slab kinds are those the fits request:
+ *   KS_PRECISION_TF32   tf32 operands, fp32 slab, tf32-rounded (round_out = 1) or unrounded (round_out = 0);
+ *   KS_PRECISION_F16    fp16 slab of the __cosf value (round_out = 1, the blocks of the fits) or of the range-reduced cosine
+ *                       (round_out = 0, their feature-mean estimates); fp16 operands, or tf32 operands when the option proj_f16 is 0;
+ *   KS_PRECISION_F16X2  split operands, round_out = 0: the unrounded fp32 slab, or with out_lo the fp16 pair (hi -> out, lo -> out_lo).
+ * Any other combination: KS_ERR_INVALID.  out / out_lo: rows x cols, row-major fp64 (ld_out); colsum_or_null (cols): the column
+ * sums the kernel accumulates for the fits' feature means. */
+KS_API int32_t ks_debug_slab(int64_t ctx, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int32_t precision, int32_t round_out,
+                             int64_t row_begin, int64_t rows, int64_t c0, int64_t cols, const double* shift_or_null, double* out,
+                             double* out_lo_or_null, int64_t ld_out, double* colsum_or_null);
+/* The residual-update / model-apply GEMM alone, launched as the fits launch it: out (M x N device matrix, updated in place)
+ * = [out +] bias + sign * acc_scale * A B^T with A (M x K), B (N x K) device matrices; apply = 0: residual update (sign -1),
+ * 1: model apply (sign +1); reduce = 1 adds into out, 0 overwrites it; bias_or_null: N values (NULL: zero); acc_scale: a power
+ * of two, read by the kernel from device memory.  precision: KS_PRECISION_TF32 (fp32 operands as they are), KS_PRECISION_F16
+ * (fp16 copies) or KS_PRECISION_F16X2 (fp16 pairs hi + lo, residual update only). */
+KS_API int32_t ks_debug_update(int64_t ctx, int64_t a, int64_t b, int32_t apply, int32_t precision, const double* bias_or_null,
+                               int32_t reduce, double acc_scale, int64_t out);
 
 /* X = H^-1 B for a symmetric positive definite H (column-major n x n) and B (column-major n x k): Cholesky with cuSOLVER, then
  * either the library's own multi-RHS solve kernel (use_cusolver = 0; option "custom_solve") or cusolverDnDpotrs (the default of

@@ -2451,12 +2451,12 @@ static void debug_split_f16(Ctx& c, Matrix& M, DevBuf& hi, DevBuf& lo) {
     c.launches += 1;
   }
 }
-static void debug_gram_run(Ctx& c, Matrix& A, Matrix& B, DevBuf& gc, int* ldg, int* ldc, DebugGramOps& ops) {
-  if (A.rows != B.rows) throw KsError{KS_ERR_INVALID, "row mismatch"};
-  ops.f16 = c.precision == KS_PRECISION_F16 || c.precision == KS_PRECISION_F16X2;
+// the kernel operands of A and B in a precision mode (KS_PRECISION_*): fp32 as they are, fp16 copies, or fp16 pairs
+static void debug_operands(Ctx& c, Matrix& A, Matrix& B, int precision, DebugGramOps& ops) {
+  ops.f16 = precision == KS_PRECISION_F16 || precision == KS_PRECISION_F16X2;
   ops.A = A.d;
   ops.B = B.d;
-  if (c.precision == KS_PRECISION_F16X2) {
+  if (precision == KS_PRECISION_F16X2) {
     debug_split_f16(c, A, ops.a16, ops.a16lo);
     debug_split_f16(c, B, ops.b16, ops.b16lo);
     ops.A = ops.a16.p;
@@ -2471,6 +2471,10 @@ static void debug_gram_run(Ctx& c, Matrix& A, Matrix& B, DevBuf& gc, int* ldg, i
     ops.A = ops.a16.p;
     ops.B = ops.b16.p;
   }
+}
+static void debug_gram_run(Ctx& c, Matrix& A, Matrix& B, DevBuf& gc, int* ldg, int* ldc, DebugGramOps& ops) {
+  if (A.rows != B.rows) throw KsError{KS_ERR_INVALID, "row mismatch"};
+  debug_operands(c, A, B, c.precision, ops);
   const int b = static_cast<int>(A.cols), kc = static_cast<int>(B.cols);
   *ldg = static_cast<int>(round_up(b, 32));
   *ldc = static_cast<int>(round_up(kc, 32));
@@ -2523,6 +2527,98 @@ KS_API int32_t ks_debug_time_gram(int64_t ctx, int64_t a, int64_t b, int32_t ite
     c.event_pool.push_back(e0);
     c.event_pool.push_back(e1);
     *out_ms = ms / std::max(iters, 1);
+  });
+}
+
+// The projection GEMM alone: the same feature source and produce_slab call as the fits, for the slab kinds they request.
+KS_API int32_t ks_debug_slab(int64_t ctx, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int32_t precision, int32_t round_out,
+                             int64_t row_begin, int64_t rows, int64_t c0, int64_t cols, const double* shift_or_null, double* out,
+                             double* out_lo_or_null, int64_t ld_out, double* colsum_or_null) {
+  return guard(ctx, [&](Ctx& c) {
+    const bool pair = out_lo_or_null != nullptr;
+    const bool f16 = precision == KS_PRECISION_F16, x2 = precision == KS_PRECISION_F16X2;
+    // tf32: fp32 slab, rounded or not; fp16 slab, rounded (the fits' blocks) or not (their mean estimates); split operands:
+    // unrounded fp32 slab or the fp16 pair
+    const bool kind_ok = (precision == KS_PRECISION_TF32 || f16) ? !pair : x2 ? round_out == 0 : false;
+    if (!kind_ok) throw KsError{KS_ERR_INVALID, "slab kind not produced by any fit"};
+    if (!out || rows <= 0 || cols <= 0 || row_begin < 0 || c0 < 0 || ld_out < cols) throw KsError{KS_ERR_INVALID, "bad slab arguments"};
+    FeatSrc src;
+    make_feat_src(c, 0, x_in, rfs, n_rfs, src, precision);
+    if (row_begin + rows > src.n_rows || c0 + cols > src.D) throw KsError{KS_ERR_INVALID, "slab window outside the features"};
+    const bool half = f16 || pair;
+    const int64_t lds = round_up(cols, 64);
+    const size_t bytes = (half ? 2 : 4) * static_cast<size_t>(rows * lds);
+    DevBuf slab, slab_lo, shift, cs;
+    slab.alloc(bytes);
+    KS_CUDA(cudaMemsetAsync(slab.p, 0, bytes, c.st));
+    if (pair) {
+      slab_lo.alloc(bytes);
+      KS_CUDA(cudaMemsetAsync(slab_lo.p, 0, bytes, c.st));
+    }
+    std::vector<float> sh32;
+    if (shift_or_null) {
+      sh32.assign(shift_or_null, shift_or_null + cols);
+      shift.alloc(sizeof(float) * static_cast<size_t>(cols));
+      KS_CUDA(cudaMemcpyAsync(shift.p, sh32.data(), sizeof(float) * cols, cudaMemcpyHostToDevice, c.st));
+    }
+    if (colsum_or_null) {
+      cs.alloc(sizeof(float) * static_cast<size_t>(cols));
+      KS_CUDA(cudaMemsetAsync(cs.p, 0, cs.bytes, c.st));
+    }
+    produce_slab(c, src, c0, cols, shift_or_null ? shift.as<float>() : src.zeros.as<float>(), slab.p, lds, row_begin, rows,
+                 round_out != 0, colsum_or_null ? cs.as<float>() : nullptr, c.st, f16, x2, pair ? slab_lo.p : nullptr);
+    c.check_async("debug_slab");
+    auto fetch = [&](const DevBuf& d, double* dst) {
+      if (half) {
+        std::vector<__half> h(static_cast<size_t>(rows * lds));
+        KS_CUDA(cudaMemcpy(h.data(), d.p, bytes, cudaMemcpyDeviceToHost));
+        for (int64_t r = 0; r < rows; ++r)
+          for (int64_t q = 0; q < cols; ++q) dst[r * ld_out + q] = __half2float(h[r * lds + q]);
+      } else {
+        std::vector<float> h(static_cast<size_t>(rows * lds));
+        KS_CUDA(cudaMemcpy(h.data(), d.p, bytes, cudaMemcpyDeviceToHost));
+        for (int64_t r = 0; r < rows; ++r)
+          for (int64_t q = 0; q < cols; ++q) dst[r * ld_out + q] = h[r * lds + q];
+      }
+    };
+    fetch(slab, out);
+    if (pair) fetch(slab_lo, out_lo_or_null);
+    if (colsum_or_null) {
+      std::vector<float> h(static_cast<size_t>(cols));
+      KS_CUDA(cudaMemcpy(h.data(), cs.p, cs.bytes, cudaMemcpyDeviceToHost));
+      for (int64_t q = 0; q < cols; ++q) colsum_or_null[q] = h[q];
+    }
+  });
+}
+
+// The residual-update / model-apply GEMM alone, through launch_update as the fits call it.
+KS_API int32_t ks_debug_update(int64_t ctx, int64_t a, int64_t b, int32_t apply, int32_t precision, const double* bias_or_null,
+                               int32_t reduce, double acc_scale, int64_t out) {
+  return guard(ctx, [&](Ctx& c) {
+    Matrix& A = c.matrix(a);
+    Matrix& B = c.matrix(b);
+    Matrix& O = c.matrix(out);
+    if (A.cols != B.cols || O.rows != A.rows || O.cols != B.rows) throw KsError{KS_ERR_INVALID, "shape mismatch"};
+    if (precision != KS_PRECISION_TF32 && precision != KS_PRECISION_F16 && precision != KS_PRECISION_F16X2)
+      throw KsError{KS_ERR_INVALID, "unsupported precision"};
+    int e = 0;
+    if (!(acc_scale > 0) || frexp(acc_scale, &e) != 0.5) throw KsError{KS_ERR_INVALID, "acc_scale must be a power of two"};
+    DebugGramOps ops;
+    debug_operands(c, A, B, precision, ops);
+    DevBuf scale, bias;
+    const float s32 = static_cast<float>(acc_scale);
+    scale.alloc(sizeof(float));
+    KS_CUDA(cudaMemcpyAsync(scale.p, &s32, sizeof(float), cudaMemcpyHostToDevice, c.st));
+    std::vector<float> b32;
+    if (bias_or_null) {
+      b32.assign(bias_or_null, bias_or_null + B.rows);
+      bias.alloc(sizeof(float) * b32.size());
+      KS_CUDA(cudaMemcpyAsync(bias.p, b32.data(), bias.bytes, cudaMemcpyHostToDevice, c.st));
+    }
+    launch_update(c, ops.A, A.ld, A.rows, static_cast<int>(A.cols), ops.B, B.ld, static_cast<int>(B.rows), O.d, O.ld,
+                  bias_or_null ? bias.as<float>() : nullptr, apply ? EPI_APPLY : EPI_UPDATE, reduce != 0, c.st, ops.f16,
+                  scale.as<float>(), ops.Alo, ops.Blo);
+    c.check_async("debug_update");
   });
 }
 
