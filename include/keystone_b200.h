@@ -317,6 +317,11 @@ KS_API int32_t ks_debug_slab(int64_t ctx, int64_t x_in, const int64_t* rfs, int3
  * (fp16 copies) or KS_PRECISION_F16X2 (fp16 pairs hi + lo, residual update only). */
 KS_API int32_t ks_debug_update(int64_t ctx, int64_t a, int64_t b, int32_t apply, int32_t precision, const double* bias_or_null,
                                int32_t reduce, double acc_scale, int64_t out);
+/* Arms the context: the next ks_blockwls_fit copies the fp64 system it assembles for class cls in feature block `block` during
+ * the first sweep, before the Cholesky factorisation overwrites it: H (b x b, column-major, b = that block's width) into
+ * H_out and the right-hand side (b) into rhs_out (either may be NULL, not both).  The host buffers must stay valid until
+ * that fit returns; the fit disarms the context whether or not the class and block exist. */
+KS_API int32_t ks_debug_bwls_capture(int64_t ctx, int32_t block, int32_t cls, double* H_out, double* rhs_out);
 
 /* X = H^-1 B for a symmetric positive definite H (column-major n x n) and B (column-major n x k): Cholesky with cuSOLVER, then
  * either the library's own multi-RHS solve kernel (use_cusolver = 0; option "custom_solve") or cusolverDnDpotrs (the default of

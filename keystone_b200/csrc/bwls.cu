@@ -16,7 +16,8 @@
 // columns are all-reduced.  Class Grams of one block are kept resident (classes_on_rank * b * b * 4 bytes).
 // Operand modes: KS_PRECISION_TF32 (one tf32 MMA per product; KS_PRECISION_F16 is accepted and computes the same way) and
 // KS_PRECISION_F16X2, the parity mode: slab, residual and increment are carried as tf32 hi + lo pairs (products keep
-// hi*hi + hi*lo + lo*hi; generated features come from the split fp16 projection), which doubles the resident class Grams.
+// hi*hi + hi*lo + lo*hi; generated features come from the split fp16 projection), which doubles the resident class Grams;
+// the diagonals of the class and population Grams are then taken in fp64 from the pairs (launch_colsumsq_pair).
 // The per-class Cholesky solves are independent: they run on kSolveLanes streams with one cuSOLVER handle each.
 #include "engine.h"
 
@@ -34,6 +35,14 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, int64_t ld, co
     const int64_t r = i / (ld / 4), c4 = i - r * (ld / 4);
     reinterpret_cast<float4*>(dst + r * ld)[c4] = reinterpret_cast<const float4*>(src + static_cast<int64_t>(perm[r]) * ld)[c4];
   }
+}
+// out[f] = sum_ci parts[ci][f]   (parts: n rows of ld doubles)
+__global__ void sum_parts_f64_kernel(const double* __restrict__ parts, int n, int64_t ld, double* __restrict__ out, int b) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= b) return;
+  double s = 0.0;
+  for (int i = 0; i < n; ++i) s += parts[static_cast<int64_t>(i) * ld + f];
+  out[f] = s;
 }
 __global__ void add_f32_kernel(const float* __restrict__ a, float* __restrict__ acc, int64_t n) {
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x)
@@ -59,10 +68,13 @@ __global__ void bwls_means_kernel(const double* __restrict__ sum, double count, 
 // H = (1-w) (Gpop/N - dp dp^T) + w (Gc/nc - dc dc^T) + w(1-w) (dc-dp)(dc-dp)^T + lam I     (:216, :248-261, :272)
 // Xpop / Xc (split-operand mode, else null): full b x b cross Grams S_hi^T S_lo; the Gram of S = S_hi + S_lo is
 // S_hi^T S_hi + X + X^T (the lo x lo term, ~2^-22 of the diagonal, is dropped)
+// diag_pop / diag_c (split-operand mode, else null): the Gram diagonals in fp64 (launch_colsumsq_pair), used instead of the
+// tensor core's, whose all-positive accumulation chains are biased low
 __global__ void bwls_build_kernel(const float* __restrict__ Gpop, const float* __restrict__ Gc, int ldg,
                                   const double* __restrict__ dp, const double* __restrict__ dc, double N, double nc, double w,
                                   double lam, double* __restrict__ H, int b, const float* __restrict__ Xpop,
-                                  const float* __restrict__ Xc) {
+                                  const float* __restrict__ Xc, const double* __restrict__ diag_pop,
+                                  const double* __restrict__ diag_c) {
   const int64_t total = static_cast<int64_t>(b) * b;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
@@ -74,6 +86,10 @@ __global__ void bwls_build_kernel(const float* __restrict__ Gpop, const float* _
       const int64_t a = static_cast<int64_t>(r) * ldg + c, t = static_cast<int64_t>(c) * ldg + r;
       gp += static_cast<double>(Xpop[a]) + static_cast<double>(Xpop[t]);
       gc += static_cast<double>(Xc[a]) + static_cast<double>(Xc[t]);
+    }
+    if (diag_pop && r == c) {
+      gp = diag_pop[r];
+      gc = diag_c[r];
     }
     const double pop = gp / N - dp[r] * dp[c];
     const double cls = gc / nc - dc[r] * dc[c];
@@ -144,6 +160,12 @@ static unsigned grid1d(int64_t n, int threads = 256) {
 
 // ------------------------------------------------------------------------------------ fit
 int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double lam, double w, int64_t nf_opt, int precision) {
+  // ks_debug_bwls_capture arms one fit: take the request and disarm before anything can throw
+  const int cap_block = c.bwls_cap_block, cap_cls = c.bwls_cap_cls;
+  double* const cap_H = c.bwls_cap_H;
+  double* const cap_rhs = c.bwls_cap_rhs;
+  c.bwls_cap_block = c.bwls_cap_cls = -1;
+  c.bwls_cap_H = c.bwls_cap_rhs = nullptr;
   if (bs <= 0 || num_iter < 1) throw KsError{KS_ERR_INVALID, "blockSize must be > 0 and numIter >= 1"};
   if (Y.rows != src.n_rows) throw KsError{KS_ERR_INVALID, "features and labels have different row counts"};
   // Multi-rank: every rank passes the rows of the classes it owns; each class must live on exactly one rank (the
@@ -255,17 +277,16 @@ int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double l
     };
     gather(Y, Yg);
     Yp = &Yg;
-    gsrc.D = src.D; gsrc.n_rows = src.n_rows; gsrc.d_in = src.d_in; gsrc.ldw = src.ldw;
-    gsrc.Wall = src.Wall; gsrc.Wfull = src.Wfull; gsrc.ball = src.ball;
     if (src.F) {
       gather(*src.F, Fg);
       gsrc.F = &Fg;
+      gsrc.D = src.D;
+      gsrc.n_rows = src.n_rows;
       gsrc.zeros.alloc(src.zeros.bytes);
       KS_CUDA(cudaMemsetAsync(gsrc.zeros.p, 0, gsrc.zeros.bytes, st));
     } else {
       gather(*src.X, Xg);
-      gsrc.X = &Xg;
-      prepare_generated_operands(c, gsrc, precision);
+      derive_feat_src(c, src, &Xg, gsrc, precision);  // the same feature map (kind included) over the gathered rows
     }
     sp = &gsrc;
   }
@@ -279,7 +300,7 @@ int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double l
   for (int cc = 0; cc < k; ++cc)
     if (gcount[cc] > 0) jlm[cc] = 2 * w + (2 * (1.0 - w) * gcount[cc] / Ntot_d) - 1;
   DevBuf jlm_d, R, Rr, Rlo, slab, slab_lo, sf32, Gcls, Xcls, Gpop, Xpop, Ctmp, Cpop, xtr, shift, negm, psum, csum, rsum_all, rsum_cls,
-      dp, dcs, dW, bop, bop_lo, cbias, fsum, facc, fail;
+      dp, dcs, dW, bop, bop_lo, cbias, fsum, facc, fail, diag_cls, diag_pop;
   jlm_d.alloc(sizeof(double) * k);
   KS_CUDA(cudaMemcpyAsync(jlm_d.p, jlm.data(), sizeof(double) * k, cudaMemcpyHostToDevice, st));
   R.alloc(sizeof(float) * static_cast<size_t>(std::max<int64_t>(N, 1) * kpad));
@@ -295,6 +316,8 @@ int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double l
     if (!sp->F) sf32.alloc(slab.bytes);
     Xcls.alloc(Gcls.bytes);
     Xpop.alloc(Gpop.bytes);
+    diag_cls.alloc(sizeof(double) * static_cast<size_t>(std::max(ncls, 1)) * lds);
+    diag_pop.alloc(sizeof(double) * lds);
   }
   Ctmp.alloc(sizeof(float) * c_elems);
   Cpop.alloc(sizeof(float) * c_elems);
@@ -426,6 +449,17 @@ int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double l
       c.launches += 2 + 2 * ncls;
       c.allreduce_f64(psum.as<double>(), static_cast<size_t>(b));
       c.allreduce_f64(rsum_all.as<double>(), static_cast<size_t>(k));
+      if (x2) {  // exact Gram diagonals (fp64) of every class range; the population's is their sum over all ranks
+        KS_CUDA(cudaMemsetAsync(diag_cls.p, 0, diag_cls.bytes, st));
+        for (int ci = 0; ci < ncls; ++ci) {
+          const Range& rg = ranges[ci];
+          launch_colsumsq_pair(slab.as<float>() + rg.off * lds, slab_lo.as<float>() + rg.off * lds, false, lds, rg.n, b,
+                               diag_cls.as<double>() + static_cast<size_t>(ci) * lds, st);
+        }
+        sum_parts_f64_kernel<<<(b + 255) / 256, 256, 0, st>>>(diag_cls.as<double>(), ncls, lds, diag_pop.as<double>(), b);
+        c.launches += ncls + 1;
+        c.allreduce_f64(diag_pop.as<double>(), static_cast<size_t>(b));
+      }
 
       // ---------------- class Grams (one tensor-core pass per class row range); population = sum of classes
       KS_CUDA(cudaMemsetAsync(Gcls.p, 0, Gcls.bytes, st));
@@ -477,13 +511,18 @@ int64_t fit_bwls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double l
         bwls_means_kernel<<<(b + 255) / 256, 256, 0, ls>>>(csum.as<double>() + static_cast<size_t>(ci) * lds, nc, dc, b);
         bwls_build_kernel<<<grid1d(static_cast<int64_t>(b) * b), 256, 0, ls>>>(
             Gpop.as<float>(), Gcls.as<float>() + static_cast<size_t>(ci) * g_elems, ldg, dp.as<double>(), dc, Ntot_d, nc, w, lam, Hq, b,
-            x2 ? Xpop.as<float>() : nullptr, x2 ? Xcls.as<float>() + static_cast<size_t>(ci) * g_elems : nullptr);
+            x2 ? Xpop.as<float>() : nullptr, x2 ? Xcls.as<float>() + static_cast<size_t>(ci) * g_elems : nullptr,
+            x2 ? diag_pop.as<double>() : nullptr, x2 ? diag_cls.as<double>() + static_cast<size_t>(ci) * lds : nullptr);
         bwls_rhs_kernel<<<(b + 255) / 256, 256, 0, ls>>>(Cpop.as<float>(), ldc, xtr.as<float>() + static_cast<size_t>(ci) * lds, m,
                                                        dp.as<double>(), dc, Ntot_d, nc, rsum_all.as<double>(),
                                                        rsum_cls.as<double>() + static_cast<size_t>(ci) * kpad, w, lam,
                                                        model->W[j]->as<double>() + static_cast<size_t>(rg.cls) * b, rq,
                                                        it == 0 ? jms[j]->as<double>() + static_cast<size_t>(rg.cls) * b : nullptr, rg.cls, b);
         c.launches += 3;
+        if (it == 0 && j == cap_block && rg.cls == cap_cls) {  // pageable destinations: these copies complete before they return
+          if (cap_H) KS_CUDA(cudaMemcpyAsync(cap_H, Hq, sizeof(double) * static_cast<size_t>(b) * b, cudaMemcpyDeviceToHost, ls));
+          if (cap_rhs) KS_CUDA(cudaMemcpyAsync(cap_rhs, rq, sizeof(double) * b, cudaMemcpyDeviceToHost, ls));
+        }
         c.lane_potrf_potrs(q, Hq, b, rq, 1, ci);
         copy_col_kernel<<<(b + 255) / 256, 256, 0, ls>>>(rq, dW.as<double>() + static_cast<size_t>(rg.cls) * b, b);
         c.launches += 1;

@@ -504,6 +504,14 @@ void make_feat_src(Ctx& c, int64_t features, int64_t x_in, const int64_t* rfs, i
   prepare_generated_operands(c, out, precision);
 }
 
+void derive_feat_src(Ctx& c, const FeatSrc& src, Matrix* X, FeatSrc& out, int precision) {
+  if (src.F || !X || X->cols != src.d_in) throw KsError{KS_ERR_INVALID, "derive_feat_src: needs a generated source and rows of its input width"};
+  static_cast<FeatMap&>(out) = static_cast<const FeatMap&>(src);
+  out.X = X;
+  out.n_rows = X->rows;
+  prepare_generated_operands(c, out, precision);
+}
+
 static void tmap16_or_throw(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols, int box_rows,
                             int swizzle) {
   const int r = make_tmap_any(m, base, rows, cols, ld, box_cols, box_rows, 2, swizzle);
@@ -2619,6 +2627,16 @@ KS_API int32_t ks_debug_update(int64_t ctx, int64_t a, int64_t b, int32_t apply,
                   bias_or_null ? bias.as<float>() : nullptr, apply ? EPI_APPLY : EPI_UPDATE, reduce != 0, c.st, ops.f16,
                   scale.as<float>(), ops.Alo, ops.Blo);
     c.check_async("debug_update");
+  });
+}
+
+KS_API int32_t ks_debug_bwls_capture(int64_t ctx, int32_t block, int32_t cls, double* H_out, double* rhs_out) {
+  return guard(ctx, [&](Ctx& c) {
+    if (block < 0 || cls < 0 || (!H_out && !rhs_out)) throw KsError{KS_ERR_INVALID, "bad arguments"};
+    c.bwls_cap_block = block;
+    c.bwls_cap_cls = cls;
+    c.bwls_cap_H = H_out;
+    c.bwls_cap_rhs = rhs_out;
   });
 }
 

@@ -217,6 +217,11 @@ struct Ctx {
   };
   std::vector<std::unique_ptr<SolveLane>> lanes;
   int solve_lanes = 4;
+  // ks_debug_bwls_capture: the next weighted fit copies the assembled fp64 system (H, rhs) of class bwls_cap_cls in block
+  // bwls_cap_block at sweep 0 to these host buffers, then disarms
+  int bwls_cap_block = -1, bwls_cap_cls = -1;
+  double* bwls_cap_H = nullptr;
+  double* bwls_cap_rhs = nullptr;
   void ensure_lanes(int n);
   // Cholesky factorisation of H (n x n, lower) + solve of nrhs right-hand sides in place, on lane q; status -> dev_info[slot]
   void lane_potrf_potrs(int q, double* H, int n, double* B, int nrhs, int info_slot);
@@ -276,8 +281,19 @@ struct Ctx {
   void check_async(const char* what);
 };
 
+// The feature map of a generated source, independent of its rows: the concatenated parameters (owned by the source they
+// were gathered for) and the map kind.  Sources over other rows of the same map copy this part whole (derive_feat_src).
+struct FeatMap {
+  float* Wall = nullptr;
+  float* Wfull = nullptr;  // unrounded fp32 weights (same layout as Wall)
+  int kind = 0;            // feature-map kind of every gathered map (CosRF::kind; mixing kinds in one gather is rejected)
+  float rect_floor = 0.f;
+  float* ball = nullptr;
+  int64_t ldw = 0, d_in = 0;
+  int64_t D = 0;
+};
 // Feature source: a materialised matrix or raw input + concatenated CosineRandomFeatures parameters.
-struct FeatSrc {
+struct FeatSrc : FeatMap {
   Matrix* F = nullptr;
   Matrix* X = nullptr;
   DevBuf xop;   // tf32-rounded copy of X (GEMM operand)
@@ -291,18 +307,14 @@ struct FeatSrc {
   int64_t ldx3 = 0, ldw3 = 0;
   bool proj_x2 = false;
   DevBuf wcat, wcat_full, bcat;
-  float* Wall = nullptr;
-  float* Wfull = nullptr;  // unrounded fp32 weights (same layout as Wall)
-  int kind = 0;            // feature-map kind of every gathered map (CosRF::kind; mixing kinds in one gather is rejected)
-  float rect_floor = 0.f;
-  float* ball = nullptr;
-  int64_t ldw = 0, d_in = 0;
-  int64_t D = 0, n_rows = 0;
+  int64_t n_rows = 0;
   DevBuf zeros;  // max(D-block, d_in) zero floats
 };
 void make_feat_src(Ctx& c, int64_t features, int64_t x_in, const int64_t* rfs, int32_t n_rfs, FeatSrc& out,
                    int precision = 0);  // KS_PRECISION_*: which operand copies of X / W to prepare
 void prepare_generated_operands(Ctx& c, FeatSrc& out, int precision);
+// out: the generated source `src` (which must outlive it) applied to the rows of X instead of its own
+void derive_feat_src(Ctx& c, const FeatSrc& src, Matrix* X, FeatSrc& out, int precision);
 // slab[rows x lds] = round_tf32(features[row_begin : row_begin+rows, c0 : c0+cols] - shift)   (shift may be the zero vector)
 // colsum (optional, fp32[cols], must be zeroed): receives the column sums of the stored slab
 // out16: the slab is fp16 (lds in fp16 elements), generated features only
