@@ -127,8 +127,37 @@ KS_API int32_t ks_cosine_rf_destroy(int64_t ctx, int64_t rf);
 KS_API int32_t ks_padded_fft_create(int64_t ctx, const double* signs_or_null, int64_t n_in, int32_t rectify, double max_val,
                                     double alpha, int64_t* out_rf);
 /* Elementwise nodes on a materialised batch: op 0: out = x .* colvec (RandomSignNode.apply), op 1: out = max(a, x - b)
- * (LinearRectifier.apply); returns a new matrix. */
+ * (LinearRectifier.apply), op 2: out = sign(x) sqrt(|x|) ((Batch)SignedHellingerMapper, K/nodes/stats/SignedHellingerMapper.scala;
+ * colvec, a and b unused); returns a new matrix. */
 KS_API int32_t ks_matrix_map(int64_t ctx, int64_t m, int32_t op, const double* colvec_or_null, double a, double b, int64_t* out_m);
+/* NormalizeRows (K/nodes/stats/NormalizeRows.scala): every row divided by max(|row|_2, 2.2e-16), the norm in fp64; a new matrix. */
+KS_API int32_t ks_matrix_normalize_rows(int64_t ctx, int64_t m, int64_t* out_m);
+
+/* ---- LCS descriptors, GMM posteriors, Fisher vectors (DESIGN.md section 16) -------------------------------------------------
+ * The LCS branch of K/pipelines/images/imagenet/ImageNetSiftLcsFV.scala.  Item batches (the reference's one DenseMatrix per image)
+ * are one device matrix with one descriptor per ROW plus item row offsets.  None of these is collective: each rank encodes its
+ * own images. */
+/* LCSExtractor(stride, strideStart, subPatchSize).apply (K/nodes/images/LCSExtractor.scala) on a batch of equal-size images, rows of
+ * `images` in ImageVectorizer order (value (x, y, c) at c + x*channels + y*channels*x_dim, x_dim = image height).  Window means and
+ * standard deviations in fp64, rounded once to fp32.  Output: (n_images * nKP) x (n^2 * channels * 2); image i owns rows
+ * [i nKP, (i+1) nKP), keypoint (xk, yk) is row xk * numPoolsY + yk, column ((c * n + nx) * n + ny) * 2 + {0: mean, 1: std}.
+ * Rejects bad shapes, no keypoint, and neighbourhoods that leave the image. */
+KS_API int32_t ks_lcs_extract(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, int32_t stride,
+                              int32_t stride_start, int32_t sub_patch_size, int64_t* out_m);
+/* GaussianMixtureModel(means, variances, weights, weightThreshold) (K/nodes/learning/GaussianMixtureModel.scala): means and variances
+ * dim x k column-major (Breeze), k weights.  Rejects non-finite values, variances <= 0, weights <= 0, dim > 1024 and a threshold
+ * outside [0, 1/k). */
+KS_API int32_t ks_gmm_create(int64_t ctx, const double* means_colmajor, const double* variances_colmajor, const double* weights,
+                             int64_t dim, int64_t k, double weight_threshold, int64_t* out_gmm);
+KS_API int32_t ks_gmm_destroy(int64_t ctx, int64_t gmm);
+/* GaussianMixtureModel.apply(X): x (N x dim) -> N x k thresholded posteriors, computed in fp64 and stored as fp32. */
+KS_API int32_t ks_gmm_posteriors(int64_t ctx, int64_t gmm, int64_t x, int64_t* out_m);
+/* FisherVector(gmm).apply andThen MatrixVectorizer (K/nodes/images/FisherVector.scala) for every item: descriptors (rows x dim), item
+ * i = rows [item_offsets[i], item_offsets[i+1]) (n_items + 1 host offsets, 0 first, rows last, strictly increasing).  Output
+ * n_items x (2 dim k) fp32, element (d, j) of the dim x 2k matrix [fv1 | fv2] at column d + dim * j.  Statistics in fp64 on the DMMA
+ * tensor core, in a fixed order (bit-reproducible); fv2 is the Sanchez et al. formula (DESIGN.md section 16). */
+KS_API int32_t ks_fisher_vector_apply(int64_t ctx, int64_t gmm, int64_t descriptors, const int64_t* item_offsets, int64_t n_items,
+                                      int64_t* out_m);
 
 /* ---- Convolver [andThen SymmetricRectifier andThen Pooler(sum) andThen ImageVectorizer] ---------------------------------
  * The featurizer of K/pipelines/images/cifar/RandomPatchCifar.scala:59-63 (K/nodes/images/Convolver.scala:20-203,

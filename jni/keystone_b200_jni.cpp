@@ -187,6 +187,47 @@ JFN(jlong, approxPcaFit)(JNIEnv* env, jobject, jlong ctx, jlong x, jdoubleArray 
   return ok(env, ctx, rc) ? h : 0;
 }
 
+// ---- LCS descriptors, GMM posteriors, Fisher vectors, row normalisation (not collective)
+JFN(jlong, lcsExtract)(JNIEnv* env, jobject, jlong ctx, jlong images, jint xDim, jint yDim, jint channels, jint stride, jint strideStart,
+                       jint subPatchSize) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_lcs_extract(ctx, images, xDim, yDim, channels, stride, strideStart, subPatchSize, &h)) ? h : 0;
+}
+// means / variances: D x K DenseMatrix.data (column-major)
+JFN(jlong, gmmCreate)(JNIEnv* env, jobject, jlong ctx, jdoubleArray means, jdoubleArray variances, jdoubleArray weights, jlong dim, jlong k,
+                      jdouble weightThreshold) {
+  int64_t h = 0;
+  jdouble* mu = env->GetDoubleArrayElements(means, nullptr);
+  jdouble* var = env->GetDoubleArrayElements(variances, nullptr);
+  jdouble* w = env->GetDoubleArrayElements(weights, nullptr);
+  const int32_t rc = (mu && var && w) ? ks_gmm_create(ctx, mu, var, w, dim, k, weightThreshold, &h) : KS_ERR_INVALID;
+  if (w) env->ReleaseDoubleArrayElements(weights, w, JNI_ABORT);
+  if (var) env->ReleaseDoubleArrayElements(variances, var, JNI_ABORT);
+  if (mu) env->ReleaseDoubleArrayElements(means, mu, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(void, gmmDestroy)(JNIEnv* env, jobject, jlong ctx, jlong gmm) { ok(env, ctx, ks_gmm_destroy(ctx, gmm)); }
+JFN(jlong, gmmPosteriors)(JNIEnv* env, jobject, jlong ctx, jlong gmm, jlong x) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_gmm_posteriors(ctx, gmm, x, &h)) ? h : 0;
+}
+// itemOffsets: nItems + 1 row offsets into the descriptor matrix
+JFN(jlong, fisherVectorApply)(JNIEnv* env, jobject, jlong ctx, jlong gmm, jlong descriptors, jlongArray itemOffsets) {
+  int64_t h = 0;
+  LongArray o(env, itemOffsets);
+  const int32_t rc = ks_fisher_vector_apply(ctx, gmm, descriptors, o.data(), o.n - 1, &h);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, matrixNormalizeRows)(JNIEnv* env, jobject, jlong ctx, jlong m) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_matrix_normalize_rows(ctx, m, &h)) ? h : 0;
+}
+// op 2 of ks_matrix_map: sign(x) sqrt(|x|)
+JFN(jlong, matrixSignedSqrt)(JNIEnv* env, jobject, jlong ctx, jlong m) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_matrix_map(ctx, m, 2, nullptr, 0.0, 0.0, &h)) ? h : 0;
+}
+
 // ---- models
 JFN(jlong, modelFromHost)(JNIEnv* env, jobject, jlong ctx, jobjectArray xs, jint blockSize, jlong k, jdoubleArray bOrNull,
                           jobjectArray meansOrNull) {

@@ -17,6 +17,16 @@ from .nodes import (  # noqa: F401
     PCATransformer,
     ZCAWhitener,
     ZCAWhitenerEstimator,
+    BatchSignedHellingerMapper,
+    FisherVector,
+    FloatToDouble,
+    GaussianMixtureModel,
+    ImageBatch,
+    ItemBatch,
+    LCSExtractor,
+    MatrixVectorizer,
+    NormalizeRows,
+    SignedHellingerMapper,
     BlockLeastSquaresEstimator,
     BlockLinearMapper,
     BlockWeightedLeastSquaresEstimator,

@@ -1797,12 +1797,19 @@ KS_API int32_t ks_padded_fft_create(int64_t ctx, const double* signs_or_null, in
     *out_rf = id;
   });
 }
-// out = x .* colvec (op 0: RandomSignNode on a batch) or max(a, x - b) (op 1: LinearRectifier on a batch), as a new matrix
+// out = x .* colvec (op 0: RandomSignNode on a batch), max(a, x - b) (op 1: LinearRectifier on a batch) or sign(x) sqrt(|x|)
+// (op 2: SignedHellingerMapper, fisher.cu), as a new matrix
 KS_API int32_t ks_matrix_map(int64_t ctx, int64_t m, int32_t op, const double* colvec_or_null, double a, double b, int64_t* out_m) {
   return guard(ctx, [&](Ctx& c) {
     Matrix& in = c.matrix(m);
-    if (!out_m || (op != 0 && op != 1) || (op == 0 && !colvec_or_null)) throw KsError{KS_ERR_INVALID, "bad matrix_map arguments"};
+    if (!out_m || (op != 0 && op != 1 && op != 2) || (op == 0 && !colvec_or_null)) throw KsError{KS_ERR_INVALID, "bad matrix_map arguments"};
     auto out = new_matrix(in.rows, in.cols);
+    if (op == 2) {
+      launch_signed_sqrt(c, in.d, out->d, in.rows * in.ld);  // padding columns stay zero
+      c.check_async("SignedHellingerMapper");
+      *out_m = c.add(std::move(out));
+      return;
+    }
     DevBuf cv64, cv32;
     if (op == 0) {
       cv64.alloc(sizeof(double) * static_cast<size_t>(in.cols));
@@ -2063,6 +2070,51 @@ KS_API int32_t ks_debug_gram_f64(int64_t ctx, int64_t a, int64_t b_or_0, const d
                                  double* out, int64_t ld_out) {
   return guard(ctx, [&](Ctx& c) {
     debug_gram_f64(c, c.matrix(a), b_or_0 ? &c.matrix(b_or_0) : nullptr, shift_a_or_null, shift_b_or_null, out, ld_out);
+  });
+}
+
+// ---------------------------------------------------------------- LCS, GMM posteriors, Fisher vectors (fisher.cu)
+static Gmm& gmm_of(Ctx& c, int64_t h) {
+  auto it = c.gmms.find(h);
+  if (it == c.gmms.end()) throw KsError{KS_ERR_HANDLE, "unknown GaussianMixtureModel handle"};
+  return *it->second;
+}
+KS_API int32_t ks_lcs_extract(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, int32_t stride,
+                              int32_t stride_start, int32_t sub_patch_size, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(lcs_extract(c, c.matrix(images), x_dim, y_dim, channels, stride, stride_start, sub_patch_size));
+  });
+}
+KS_API int32_t ks_gmm_create(int64_t ctx, const double* means_colmajor, const double* variances_colmajor, const double* weights, int64_t dim,
+                             int64_t k, double weight_threshold, int64_t* out_gmm) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_gmm) throw KsError{KS_ERR_INVALID, "null out_gmm"};
+    *out_gmm = gmm_create(c, means_colmajor, variances_colmajor, weights, dim, k, weight_threshold);
+  });
+}
+KS_API int32_t ks_gmm_destroy(int64_t ctx, int64_t gmm) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!c.gmms.erase(gmm)) throw KsError{KS_ERR_HANDLE, "unknown GaussianMixtureModel handle"};
+  });
+}
+KS_API int32_t ks_gmm_posteriors(int64_t ctx, int64_t gmm, int64_t x, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(gmm_posteriors(c, gmm_of(c, gmm), c.matrix(x)));
+  });
+}
+KS_API int32_t ks_fisher_vector_apply(int64_t ctx, int64_t gmm, int64_t descriptors, const int64_t* item_offsets, int64_t n_items,
+                                      int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(fisher_vector_apply(c, gmm_of(c, gmm), c.matrix(descriptors), item_offsets, n_items));
+  });
+}
+KS_API int32_t ks_matrix_normalize_rows(int64_t ctx, int64_t m, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(normalize_rows(c, c.matrix(m)));
   });
 }
 

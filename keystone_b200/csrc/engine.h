@@ -123,6 +123,19 @@ struct GaussKernel {
   DevBuf scale;  // fp32 [2]: 2^e, 2^-e
 };
 
+// GaussianMixtureModel(means, variances, weights, weightThreshold) (K/nodes/learning/GaussianMixtureModel.scala): fp64 parameters on
+// the device for the posteriors and the Fisher vectors (fisher.cu, DESIGN.md section 16)
+struct Gmm {
+  int64_t dim = 0, k = 0;
+  double thr = 1e-4;
+  DevBuf buf;  // [mu | var | 0.5 / var] each dim x k row-major ([d][k]), then ck[k] = log w - 1/2 sum_d log var - dim/2 log 2 pi, w[k]
+  const double* mu() const { return buf.as<double>(); }
+  const double* var() const { return mu() + dim * k; }
+  const double* hiv() const { return mu() + 2 * dim * k; }
+  const double* ck() const { return mu() + 3 * dim * k; }
+  const double* w() const { return ck() + k; }
+};
+
 struct Model {  // BlockLinearMapper state (K/nodes/learning/BlockLinearMapper.scala:22-33)
   std::shared_ptr<GaussKernel> kernel;  // KernelBlockLinearMapper (K/nodes/learning/KernelBlockLinearMapper.scala): the training rows
   int block_size = 0;
@@ -247,6 +260,7 @@ struct Ctx {
   std::unordered_map<int64_t, std::unique_ptr<Model>> models;
   std::unordered_map<int64_t, std::unique_ptr<ConvPool>> convs;
   std::unordered_map<int64_t, std::shared_ptr<GaussKernel>> kernels;
+  std::unordered_map<int64_t, std::unique_ptr<Gmm>> gmms;
   std::map<std::vector<int>, std::unique_ptr<DevBuf>> tile_cache;
   // phase timing of the current fit
   struct Span { int phase; cudaEvent_t a, b; int stream; };
@@ -365,5 +379,15 @@ int64_t approx_range(Ctx& c, Matrix& X, const double* omega_colmajor, int l, int
 int64_t fit_approx_pca(Ctx& c, Matrix& X, const double* omega_colmajor, int dims, int q, int p);
 // out (m x n, row-major fp64, host) = (A - 1 s^T)^T (B - 1 t^T); B null: symmetric mode.  Not collective.
 void debug_gram_f64(Ctx& c, Matrix& A, Matrix* B, const double* shift_a, const double* shift_b, double* out, int64_t ld_out);
+
+// LCS descriptors, GMM posteriors, Fisher vectors and row normalisation (fisher.cu); none is collective
+std::unique_ptr<Matrix> lcs_extract(Ctx& c, Matrix& images, int x_dim, int y_dim, int channels, int stride, int stride_start,
+                                    int sub_patch_size);
+int64_t gmm_create(Ctx& c, const double* means_colmajor, const double* vars_colmajor, const double* weights, int64_t dim, int64_t k,
+                   double weight_threshold);
+std::unique_ptr<Matrix> gmm_posteriors(Ctx& c, const Gmm& g, Matrix& X);
+std::unique_ptr<Matrix> fisher_vector_apply(Ctx& c, const Gmm& g, Matrix& X, const int64_t* item_offsets, int64_t n_items);
+std::unique_ptr<Matrix> normalize_rows(Ctx& c, Matrix& in);
+void launch_signed_sqrt(Ctx& c, const float* in, float* out, int64_t n);
 
 }  // namespace ks

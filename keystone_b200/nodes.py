@@ -893,6 +893,10 @@ class BatchPCATransformer(Transformer):
         return self.transformer.pca_mat
 
     def apply(self, data):
+        if isinstance(data, ItemBatch):  # device items (LCSExtractor output): one apply over all rows, offsets kept
+            if data.cols != self.pca_mat.shape[0]:
+                raise ValueError(f"every item must have {self.pca_mat.shape[0]} rows")
+            return ItemBatch(self.transformer.apply(data.matrix), data.offsets)
         single = isinstance(data, np.ndarray) and data.ndim == 2
         items = [np.asarray(data)] if single else [np.asarray(m) for m in data]
         d = self.pca_mat.shape[0]
@@ -1111,3 +1115,263 @@ class StandardScalerModel(Transformer):
 
     def __init__(self, mean: np.ndarray, std: Optional[np.ndarray] = None):
         self.mean, self.std = mean, std
+
+
+# ------------------------------------------------------------------------------------------ LCS Fisher-vector branch
+# LCSExtractor -> BatchPCATransformer -> FisherVector(gmm) -> FloatToDouble -> MatrixVectorizer -> NormalizeRows -> SignedHellingerMapper
+# -> NormalizeRows (K/pipelines/images/imagenet/ImageNetSiftLcsFV.scala).  DESIGN.md section 16.
+class ItemBatch(Dataset):
+    """A batch of items -- the reference's one (dim x n_i) ``DenseMatrix[Float]`` per image -- as ONE device matrix holding the columns
+    of every item as rows, plus item row offsets: item i is rows [offsets[i], offsets[i + 1])."""
+
+    def __init__(self, matrix: DeviceMatrix, offsets):
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        if offsets.ndim != 1 or offsets.size < 1 or offsets[0] != 0 or offsets[-1] != matrix.rows or (np.diff(offsets) < 0).any():
+            raise ValueError("item offsets must start at 0, end at the row count and never decrease")
+        self.ctx, self.matrix, self.offsets = matrix.ctx, matrix, offsets
+
+    @classmethod
+    def from_items(cls, ctx: Context, items: Sequence[np.ndarray]) -> "ItemBatch":
+        """Uploads (dim x n_i) host matrices."""
+        items = [np.atleast_2d(np.asarray(m)) for m in items]
+        offsets = np.cumsum([0] + [m.shape[1] for m in items])
+        return cls(ctx.matrix(np.concatenate([m.T for m in items], 0).astype(np.float32)), offsets)
+
+    @property
+    def n_items(self) -> int:
+        return int(self.offsets.size - 1)
+
+    @property
+    def rows(self) -> int:
+        return self.matrix.rows
+
+    @property
+    def cols(self) -> int:
+        return self.matrix.cols
+
+    def to_list(self, dtype=np.float64) -> List[np.ndarray]:
+        """The items as the reference's (dim x n_i) matrices."""
+        host = self.matrix.to_numpy(dtype)
+        return [np.ascontiguousarray(host[self.offsets[i]:self.offsets[i + 1]].T) for i in range(self.n_items)]
+
+    def to_numpy(self, dtype=np.float64) -> np.ndarray:
+        return self.matrix.to_numpy(dtype)
+
+
+class ImageBatch(Dataset):
+    """Equal-size images as rows of a device matrix in ImageVectorizer order (value (x, y, c) at c + x*C + y*C*xDim, x = row)."""
+
+    def __init__(self, matrix: DeviceMatrix, x_dim: int, y_dim: int, channels: int):
+        if matrix.cols != x_dim * y_dim * channels:
+            raise ValueError("image matrix columns must equal x_dim * y_dim * channels")
+        self.ctx, self.matrix = matrix.ctx, matrix
+        self.x_dim, self.y_dim, self.channels = int(x_dim), int(y_dim), int(channels)
+
+    @classmethod
+    def from_images(cls, ctx: Context, images_xyc: np.ndarray) -> "ImageBatch":
+        """(n, x, y, c) host images."""
+        a = np.asarray(images_xyc)
+        return cls(ctx.matrix(images_to_matrix(a)), a.shape[1], a.shape[2], a.shape[3])
+
+    @property
+    def rows(self) -> int:
+        return self.matrix.rows
+
+
+class LCSExtractor(Transformer):
+    """``new LCSExtractor(stride, strideStart, subPatchSize)`` (K/nodes/images/LCSExtractor.scala): per keypoint, the mean and standard
+    deviation of every channel over n x n neighbouring s x s windows (96 values for 3 channels and the defaults).  Window statistics in
+    fp64, rounded once to fp32.  Input: an ``ImageBatch``, an (n, x, y, c) array, one (x, y, c) image (returns its (dim x nKP) matrix)
+    or a list of images, grouped by shape.  Output: an ``ItemBatch`` with one item per image."""
+
+    def __init__(self, stride: int, strideStart: int, subPatchSize: int, ctx: Optional[Context] = None):
+        self.stride, self.stride_start, self.sub_patch_size, self.ctx = int(stride), int(strideStart), int(subPatchSize), ctx
+
+    def keypoints(self, x_dim: int, y_dim: int) -> int:
+        return len(range(self.stride_start, x_dim - self.stride_start, self.stride)) * \
+            len(range(self.stride_start, y_dim - self.stride_start, self.stride))
+
+    def _extract(self, batch: ImageBatch) -> ItemBatch:
+        h = C.c_int64(0)
+        check(batch.ctx.handle, lib().ks_lcs_extract(batch.ctx.handle, batch.matrix.handle, batch.x_dim, batch.y_dim, batch.channels,
+                                                      self.stride, self.stride_start, self.sub_patch_size, C.byref(h)))
+        rows, cols = C.c_int64(0), C.c_int64(0)
+        check(batch.ctx.handle, lib().ks_matrix_shape(batch.ctx.handle, h.value, C.byref(rows), C.byref(cols)))
+        nkp = self.keypoints(batch.x_dim, batch.y_dim)
+        return ItemBatch(DeviceMatrix(batch.ctx, h.value, rows.value, cols.value), np.arange(batch.rows + 1, dtype=np.int64) * nkp)
+
+    def apply(self, data):
+        if isinstance(data, ImageBatch):
+            return self._extract(data)
+        if self.ctx is None:
+            raise KeystoneError(-1, "numpy input needs a Context (pass ctx= to the node)")
+        if isinstance(data, np.ndarray) and data.ndim == 3:
+            return self._extract(ImageBatch.from_images(self.ctx, data[None])).to_list(np.float32)[0]
+        if isinstance(data, np.ndarray) and data.ndim == 4:
+            return self._extract(ImageBatch.from_images(self.ctx, data))
+        images = [np.asarray(im) for im in data]
+        groups = {}
+        for i, im in enumerate(images):
+            groups.setdefault(im.shape, []).append(i)
+        if len(groups) == 1:
+            return self._extract(ImageBatch.from_images(self.ctx, np.stack(images)))
+        # several shapes: one launch per shape, the items put back in input order on the host
+        items: List[Optional[np.ndarray]] = [None] * len(images)
+        for idx in groups.values():
+            for i, m in zip(idx, self._extract(ImageBatch.from_images(self.ctx, np.stack([images[i] for i in idx]))).to_list(np.float32)):
+                items[i] = m
+        return ItemBatch.from_items(self.ctx, items)
+
+
+class _GmmHandle:
+    def __init__(self, ctx: Context, handle: int):
+        self.ctx, self.handle = ctx, handle
+
+    def __del__(self):
+        try:
+            if self.handle and self.ctx.handle:
+                lib().ks_gmm_destroy(self.ctx.handle, self.handle)
+        except Exception:
+            pass
+
+
+class GaussianMixtureModel(Transformer):
+    """``GaussianMixtureModel(means, variances, weights, weightThreshold)`` (K/nodes/learning/GaussianMixtureModel.scala): means and
+    variances are dim x k (one column per component).  ``apply`` returns the thresholded posteriors, computed in fp64 on the device:
+    a vector for a vector, a device batch (N x k) for a batch.  The device copy is made per Context, on first use or when ``ctx`` is
+    given."""
+
+    def __init__(self, means, variances, weights, weightThreshold: float = 1e-4, ctx: Optional[Context] = None):
+        self.means = np.asarray(means, dtype=np.float64)
+        self.variances = np.asarray(variances, dtype=np.float64)
+        self.weights = np.asarray(weights, dtype=np.float64).reshape(-1)
+        if self.means.ndim != 2 or self.means.shape != self.variances.shape:
+            raise ValueError("GMM means and variances must be the same size.")
+        if self.weights.size != self.means.shape[1]:
+            raise ValueError("Every GMM center must have a weight.")
+        self.weight_threshold, self.ctx = float(weightThreshold), ctx
+        self._handles = {}
+        if ctx is not None:
+            self.handle(ctx)
+
+    @property
+    def dim(self) -> int:
+        return self.means.shape[0]
+
+    @property
+    def k(self) -> int:
+        return self.means.shape[1]
+
+    @classmethod
+    def load(cls, meanFile: str, varsFile: str, weightsFile: str, ctx: Optional[Context] = None) -> "GaussianMixtureModel":
+        """``GaussianMixtureModel.load`` (GaussianMixtureModel.scala:95-105): headerless CSVs, means and variances dim x k; the weights
+        file flattened column-major (csvread(...).toDenseVector)."""
+        from .loaders import CsvDataLoader
+        w = CsvDataLoader(weightsFile, np.float64).reshape(-1, order="F")
+        return cls(CsvDataLoader(meanFile, np.float64), CsvDataLoader(varsFile, np.float64), w, ctx=ctx)
+
+    def handle(self, ctx: Context) -> int:
+        owner = self._handles.get(ctx.handle)
+        if owner is None:
+            m, v = np.asfortranarray(self.means), np.asfortranarray(self.variances)
+            w = np.ascontiguousarray(self.weights)
+            h = C.c_int64(0)
+            check(ctx.handle, lib().ks_gmm_create(ctx.handle, m.ctypes.data_as(C.c_void_p), v.ctypes.data_as(C.c_void_p),
+                                                   w.ctypes.data_as(C.c_void_p), self.dim, self.k, self.weight_threshold, C.byref(h)))
+            owner = self._handles[ctx.handle] = _GmmHandle(ctx, h.value)
+        return owner.handle
+
+    def apply(self, data):
+        single = isinstance(data, np.ndarray) and data.ndim == 1
+        x = _device_matrix(self.ctx, data)
+        h = C.c_int64(0)
+        check(x.ctx.handle, lib().ks_gmm_posteriors(x.ctx.handle, self.handle(x.ctx), x.handle, C.byref(h)))
+        out = DeviceMatrix(x.ctx, h.value, x.rows, self.k)
+        return out.to_numpy()[0] if single else out
+
+
+class FisherVector(Transformer):
+    """``FisherVector(gmm)`` (K/nodes/images/FisherVector.scala) followed by MatrixVectorizer: one row of 2 dim k values per item,
+    element (d, j) of the reference's dim x 2k matrix [fv1 | fv2] at column d + dim * j.  Posteriors and statistics stay on the
+    device in fp64; the output is fp32.  fv2 follows Sanchez et al. (DESIGN.md section 16).  Input: an ``ItemBatch``, a list of
+    (dim x n_i) matrices, or one such matrix (returns its dim x 2k matrix)."""
+
+    def __init__(self, gmm: GaussianMixtureModel):
+        self.gmm = gmm
+
+    def apply(self, data):
+        single = isinstance(data, np.ndarray) and data.ndim == 2
+        if not isinstance(data, ItemBatch):
+            ctx = self.gmm.ctx
+            if ctx is None:
+                raise KeystoneError(-1, "host items need a Context (pass ctx= to the GaussianMixtureModel)")
+            data = ItemBatch.from_items(ctx, [data] if single else list(data))
+        ctx = data.ctx
+        offs = data.offsets
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_fisher_vector_apply(ctx.handle, self.gmm.handle(ctx), data.matrix.handle, offs.ctypes.data_as(C.c_void_p),
+                                                        data.n_items, C.byref(h)))
+        out = DeviceMatrix(ctx, h.value, data.n_items, 2 * self.gmm.dim * self.gmm.k)
+        if single:
+            return out.to_numpy()[0].reshape(2 * self.gmm.k, self.gmm.dim).T.copy()
+        return out
+
+
+class FloatToDouble(Transformer):
+    """K/nodes/util/FloatToDouble: device storage is fp32 and every consumer computes in fp64, so this passes its input through."""
+
+    def apply(self, data):
+        return data
+
+
+class MatrixVectorizer(Transformer):
+    """K/nodes/util/MatrixVectorizer: ``FisherVector`` already writes each item's matrix column-major as one row, so this passes its
+    input through."""
+
+    def apply(self, data):
+        return data
+
+
+def _map_rows(data, ctx: Optional[Context], fn) -> object:
+    """Applies a device row map to a batch (DeviceMatrix, ItemBatch: offsets kept) or a host vector / matrix."""
+    if isinstance(data, ItemBatch):
+        return ItemBatch(fn(data.matrix), data.offsets)
+    single = isinstance(data, np.ndarray) and data.ndim == 1
+    out = fn(_device_matrix(ctx, data))
+    return out.to_numpy()[0] if single else out
+
+
+def _normalize_rows(x: DeviceMatrix) -> DeviceMatrix:
+    h = C.c_int64(0)
+    check(x.ctx.handle, lib().ks_matrix_normalize_rows(x.ctx.handle, x.handle, C.byref(h)))
+    return DeviceMatrix(x.ctx, h.value, x.rows, x.cols)
+
+
+def _signed_sqrt(x: DeviceMatrix) -> DeviceMatrix:
+    h = C.c_int64(0)
+    check(x.ctx.handle, lib().ks_matrix_map(x.ctx.handle, x.handle, 2, None, 0.0, 0.0, C.byref(h)))
+    return DeviceMatrix(x.ctx, h.value, x.rows, x.cols)
+
+
+class NormalizeRows(Transformer):
+    """NormalizeRows (K/nodes/stats/NormalizeRows.scala): each row divided by max(|row|_2, 2.2e-16), the norm in fp64."""
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx
+
+    def apply(self, data):
+        return _map_rows(data, self.ctx, _normalize_rows)
+
+
+class SignedHellingerMapper(Transformer):
+    """SignedHellingerMapper (K/nodes/stats/SignedHellingerMapper.scala): sign(v) sqrt(|v|) elementwise."""
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx
+
+    def apply(self, data):
+        return _map_rows(data, self.ctx, _signed_sqrt)
+
+
+class BatchSignedHellingerMapper(SignedHellingerMapper):
+    """BatchSignedHellingerMapper: the same map on (dim x n) Float items (an ``ItemBatch`` keeps its offsets)."""

@@ -39,6 +39,17 @@ class KeystoneB200 extends Serializable {
   @native def zcaFit(ctx: Long, x: Long, eps: Double): Long
   @native def approxRange(ctx: Long, x: Long, omega: Array[Double], l: Int, q: Int): Long
   @native def approxPcaFit(ctx: Long, x: Long, omega: Array[Double], dims: Int, q: Int, p: Int): Long
+  /** LCS descriptors, GMM posteriors, Fisher vectors (not collective; DESIGN.md section 16).  means / variances: D x K
+   *  DenseMatrix.data; itemOffsets: nItems + 1 row offsets into the descriptor matrix. */
+  @native def lcsExtract(ctx: Long, images: Long, xDim: Int, yDim: Int, channels: Int, stride: Int, strideStart: Int,
+      subPatchSize: Int): Long
+  @native def gmmCreate(ctx: Long, means: Array[Double], variances: Array[Double], weights: Array[Double], dim: Long, k: Long,
+      weightThreshold: Double): Long
+  @native def gmmDestroy(ctx: Long, gmm: Long): Unit
+  @native def gmmPosteriors(ctx: Long, gmm: Long, x: Long): Long
+  @native def fisherVectorApply(ctx: Long, gmm: Long, descriptors: Long, itemOffsets: Array[Long]): Long
+  @native def matrixNormalizeRows(ctx: Long, m: Long): Long
+  @native def matrixSignedSqrt(ctx: Long, m: Long): Long
 
   @native def modelFromHost(ctx: Long, xs: Array[Array[Double]], blockSize: Int, k: Long, b: Array[Double],
       means: Array[Array[Double]]): Long
