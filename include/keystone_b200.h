@@ -339,6 +339,15 @@ KS_API int32_t ks_debug_gram_f64(int64_t ctx, int64_t a, int64_t b_or_0, const d
 KS_API int32_t ks_debug_slab(int64_t ctx, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int32_t precision, int32_t round_out,
                              int64_t row_begin, int64_t rows, int64_t c0, int64_t cols, const double* shift_or_null, double* out,
                              double* out_lo_or_null, int64_t ld_out, double* colsum_or_null);
+/* Times `iters` launches of the projection alone (CUDA events; returns ms per launch): feature columns [0, cols) of all rows of
+ * x_in + rfs[n_rfs], the slab kind as in ks_debug_slab (shift zero), launched as a block fit's first sweep launches it (on the
+ * look-ahead stream, column sums on; for the fp16 pair also the exact Gram diagonal).  diag_or_null (KS_PRECISION_F16X2 only,
+ * cols values): the fp64 sum of (hi + lo)^2 per column accumulated by the last launch.  out_or_null / out_lo_or_null (rows x cols,
+ * row-major fp64): the slab of the last launch (the lo plane for KS_PRECISION_F16X2 only).  The option reserve_sms sets how many
+ * SMs the launch leaves free, as in the fits. */
+KS_API int32_t ks_debug_time_slab(int64_t ctx, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int32_t precision, int32_t round_out,
+                                  int64_t cols, int32_t iters, double* out_ms, double* diag_or_null, double* out_or_null,
+                                  double* out_lo_or_null);
 /* The residual-update / model-apply GEMM alone, launched as the fits launch it: out (M x N device matrix, updated in place)
  * = [out +] bias + sign * acc_scale * A B^T with A (M x K), B (N x K) device matrices; apply = 0: residual update (sign -1),
  * 1: model apply (sign +1); reduce = 1 adds into out, 0 overwrites it; bias_or_null: N values (NULL: zero); acc_scale: a power

@@ -134,6 +134,7 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_debug_time_gram", i64, i64, i64, i32, p_f64)
     sig("ks_debug_chol_solve", i64, C.c_void_p, i32, C.c_void_p, i32, i32, C.c_void_p, p_f64)
     sig("ks_debug_slab", i64, i64, p_i64, i32, i32, i32, i64, i64, i64, i64, C.c_void_p, C.c_void_p, C.c_void_p, i64, C.c_void_p)
+    sig("ks_debug_time_slab", i64, i64, p_i64, i32, i32, i32, i64, i32, p_f64, C.c_void_p, C.c_void_p, C.c_void_p)
     sig("ks_debug_update", i64, i64, i64, i32, i32, C.c_void_p, i32, f64, i64)
     sig("ks_debug_bwls_capture", i64, i32, i32, C.c_void_p, C.c_void_p)
 

@@ -528,8 +528,10 @@ static void tmap_or_throw(CUtensorMap* m, const float* base, int64_t rows, int64
 }
 
 void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* shift, void* slab_v, int64_t lds,
-                  int64_t row_begin, int64_t rows, bool round_out, float* colsum, cudaStream_t st, bool out16, bool x2, void* slab_lo) {
+                  int64_t row_begin, int64_t rows, bool round_out, float* colsum, cudaStream_t st, bool out16, bool x2, void* slab_lo,
+                  double* colsumsq) {
   if (rows <= 0 || cols <= 0) return;
+  if (colsumsq && (!slab_lo || !colsum)) throw KsError{KS_ERR_INVALID, "the exact diagonal comes with the fp16 pair's column sums"};
   if (!st) st = c.st;
   float* slab = static_cast<float*>(slab_v);
   if (src.F) {
@@ -571,6 +573,7 @@ void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* s
   k.p.vec0 = src.ball + c0;
   k.p.vec1 = shift;
   k.p.colsum = colsum;
+  k.p.colsumsq = colsumsq;
   k.p.M = static_cast<int>(rows);
   k.p.N = static_cast<int>(cols);
   k.p.K = static_cast<int>(kdepth);
@@ -975,9 +978,10 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
       launch_center_round(src.F->d, src.F->ld, static_cast<int>(c0), shifts[j]->as<float>(), slab[buf].as<float>(), cs, lds, n_loc, b,
                           ST, slab_lo[buf].as<float>());
       c.launches += 1;
-    } else if (x2 && f16) {  // fp16 pairs straight out of the projection's epilogue
+    } else if (x2 && f16) {  // fp16 pairs straight out of the projection's epilogue, with the exact diagonal on the first sweep
+      if (cs) KS_CUDA(cudaMemsetAsync(dsq[buf].p, 0, dsq[buf].bytes, ST));
       produce_slab(c, src, c0, b, shifts[j]->as<float>(), slab[buf].p, lds, 0, n_loc, /*round_out=*/false, cs, ST, false, true,
-                   slab_lo[buf].p);
+                   slab_lo[buf].p, cs ? dsq[buf].as<double>() : nullptr);
       flops += 4.0 * static_cast<double>(n_loc) * src.d_in * b;  // two extra product terms of the projection
     } else if (x2) {
       produce_slab(c, src, c0, b, shifts[j]->as<float>(), sf32.p, lds, 0, n_loc, /*round_out=*/false, nullptr, ST, false, true);
@@ -989,7 +993,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
       produce_slab(c, src, c0, b, shifts[j]->as<float>(), slab[buf].p, lds, 0, n_loc, true, cs, ST, f16);
     }
     if (!src.F) flops += 2.0 * static_cast<double>(n_loc) * src.d_in * b;
-    if (x2 && it == 0) {  // the diagonal of this block's Gram matrix, exactly (the tensor core's is biased low: aux_kernels.cu)
+    if (x2 && !f16 && it == 0) {  // tf32 pairs: the diagonal of this block's Gram matrix, exactly (the tensor core's is biased low)
       KS_CUDA(cudaMemsetAsync(dsq[buf].p, 0, dsq[buf].bytes, ST));
       launch_colsumsq_pair(slab[buf].p, slab_lo[buf].p, f16, lds, n_loc, b, dsq[buf].as<double>(), ST);
       c.launches += 1;
@@ -2648,6 +2652,66 @@ KS_API int32_t ks_debug_slab(int64_t ctx, int64_t x_in, const int64_t* rfs, int3
       KS_CUDA(cudaMemcpy(h.data(), cs.p, cs.bytes, cudaMemcpyDeviceToHost));
       for (int64_t q = 0; q < cols; ++q) colsum_or_null[q] = h[q];
     }
+  });
+}
+
+// The projection alone, timed: the block fit's first-sweep produce_slab call (column sums on, and for the fp16 pair the exact
+// diagonal) on the look-ahead stream, so with the same SM count and tile schedule as in the fit.
+KS_API int32_t ks_debug_time_slab(int64_t ctx, int64_t x_in, const int64_t* rfs, int32_t n_rfs, int32_t precision, int32_t round_out,
+                                  int64_t cols, int32_t iters, double* out_ms, double* diag_or_null, double* out_or_null,
+                                  double* out_lo_or_null) {
+  return guard(ctx, [&](Ctx& c) {
+    const bool f16 = precision == KS_PRECISION_F16, x2 = precision == KS_PRECISION_F16X2;
+    const bool kind_ok = precision == KS_PRECISION_TF32 || f16 || (x2 && round_out == 0);
+    if (!kind_ok) throw KsError{KS_ERR_INVALID, "slab kind not produced by any fit"};
+    if (!out_ms || cols <= 0 || iters <= 0) throw KsError{KS_ERR_INVALID, "bad slab timing arguments"};
+    if (diag_or_null && !x2) throw KsError{KS_ERR_INVALID, "the exact diagonal comes with the fp16 pair only"};
+    FeatSrc src;
+    make_feat_src(c, 0, x_in, rfs, n_rfs, src, precision);
+    if (cols > src.D) throw KsError{KS_ERR_INVALID, "more columns than features"};
+    const int64_t rows = src.n_rows, lds = round_up(cols, 64);
+    const size_t bytes = ((f16 || x2) ? 2 : 4) * static_cast<size_t>(rows * lds);
+    DevBuf slab, slab_lo, cs, dg;
+    slab.alloc(bytes);
+    if (x2) slab_lo.alloc(bytes);
+    cs.alloc(sizeof(float) * static_cast<size_t>(cols));
+    if (x2) dg.alloc(sizeof(double) * static_cast<size_t>(cols));
+    cudaStream_t st = c.st2;
+    KS_CUDA(cudaStreamSynchronize(c.st));  // the feature source's operands are prepared on the main stream
+    auto run = [&]() {
+      KS_CUDA(cudaMemsetAsync(cs.p, 0, cs.bytes, st));
+      if (x2) KS_CUDA(cudaMemsetAsync(dg.p, 0, dg.bytes, st));
+      produce_slab(c, src, 0, cols, src.zeros.as<float>(), slab.p, lds, 0, rows, round_out != 0, cs.as<float>(), st, f16, x2,
+                   x2 ? slab_lo.p : nullptr, x2 ? dg.as<double>() : nullptr);
+    };
+    run();  // warm-up
+    cudaEvent_t e0 = c.get_event(), e1 = c.get_event();
+    KS_CUDA(cudaEventRecord(e0, st));
+    for (int i = 0; i < iters; ++i) run();
+    KS_CUDA(cudaEventRecord(e1, st));
+    KS_CUDA(cudaStreamSynchronize(st));
+    c.check_async("debug_time_slab");
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    c.event_pool.push_back(e0);
+    c.event_pool.push_back(e1);
+    *out_ms = ms / iters;
+    if (diag_or_null) KS_CUDA(cudaMemcpy(diag_or_null, dg.p, dg.bytes, cudaMemcpyDeviceToHost));
+    auto fetch = [&](const DevBuf& d, double* dst) {
+      if (f16 || x2) {
+        std::vector<__half> h(static_cast<size_t>(rows * lds));
+        KS_CUDA(cudaMemcpy(h.data(), d.p, bytes, cudaMemcpyDeviceToHost));
+        for (int64_t r = 0; r < rows; ++r)
+          for (int64_t q = 0; q < cols; ++q) dst[r * cols + q] = __half2float(h[r * lds + q]);
+      } else {
+        std::vector<float> h(static_cast<size_t>(rows * lds));
+        KS_CUDA(cudaMemcpy(h.data(), d.p, bytes, cudaMemcpyDeviceToHost));
+        for (int64_t r = 0; r < rows; ++r)
+          for (int64_t q = 0; q < cols; ++q) dst[r * cols + q] = h[r * lds + q];
+      }
+    };
+    if (out_or_null) fetch(slab, out_or_null);
+    if (out_lo_or_null && x2) fetch(slab_lo, out_lo_or_null);
   });
 }
 

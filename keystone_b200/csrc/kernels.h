@@ -40,7 +40,13 @@ struct KmParams {
   // EPI_POOL (Convolver -> SymmetricRectifier -> sum Pooler -> ImageVectorizer, fused): rows are image patches (patches_per_image
   // consecutive rows per image), columns are filters; out[img][pool * 2 N + {0, N} + filter] += max(floor, +-acc - alpha)
   const unsigned* pool_mask = nullptr;  // [patches_per_image] bit p set: the patch position lies in pool p (pools may overlap)
-  float* pool_out = nullptr;
+  union {
+    float* pool_out = nullptr;
+    // EPI_COS with the fp16 pair output (out16 == 2) and colsum: if non-null, colsumsq[n] += sum over valid rows of (hi + lo)^2
+    // in fp64, the exact Gram diagonal of the slab.  It shares pool_out's slot so that KmParams, and with it the code of every
+    // other instantiation, stays as it was.
+    double* colsumsq;
+  };
   int64_t pool_out_ld = 0;
   int patches_per_image = 0, n_pools = 0;
   float pool_alpha = 0.f;

@@ -19,6 +19,8 @@
 // epilogue math -> 128 B-swizzled staging -> TMA store / TMA reduce-add, so global memory only sees full 128 B rows.
 // wgmma accepts tf32 operands only K-major, so the tf32 Gram (MN-major) builds warp-level mma.sync fragments from the same
 // TMA-filled stages instead.
+// The slab producers (EPI_COS, EPI_RBF) add a fourth warpgroup that runs the epilogue while the MMA warpgroups go on to the next
+// tile (KmSmem).
 // SPLIT variants (parity mode, fp16 pairs; Gram and EPI_UPDATE): each stage holds the hi and lo planes of both operands and one
 // pass issues hi·hi, lo·hi and hi·lo into two accumulators, so the operands are fetched and the output is reduce-added once.
 #include <type_traits>
@@ -63,6 +65,54 @@ __device__ __forceinline__ SmemLayout carve_smem(uint8_t* smem_raw) {
   return L;
 }
 
+// Slab producers (EPI_COS, EPI_RBF) run their epilogue in separate warps, so that the MMA warpgroups go straight on to the next
+// tile: they dump the accumulator into a whole-tile fp32 buffer and hand it over with the tile id (tile_full), and the epilogue
+// warps give the buffer back (tile_empty) once they have read it.  Their epilogue per element (range-reduced cosine or exp, the
+// hi / lo split, the fp16 staging, column sums) costs about as much as the tile's MMA at K ~ 1000, so it now hides under the next
+// tile's main loop.  Eight epilogue warps, two per SM sub-partition (one warp each leaves the epilogue's latencies exposed and
+// makes it slower than the MMA): the three warps of the producer warpgroup that issue no TMA, warpgroup 3 and a 17th warp, 544
+// threads (120 registers each).  Each takes two 32 x 32 chunks of a tile.  Shared memory: 4 stages, the 128 x 129 tile buffer,
+// one 4 KB staging chunk per epilogue warp and one copy of the tile's vec0 / vec1 columns for all of them.
+__host__ __device__ constexpr bool km_async(int epi) { return epi == EPI_COS || epi == EPI_RBF; }
+__host__ __device__ constexpr int km_threads(int epi) { return km_async(epi) ? 544 : kThreads; }
+static constexpr int kEpiWarps = 8;
+static constexpr int kTileLd = 129;  // odd row pitch, as kRawLd
+static constexpr int kTileBufBytes = kTileM * kTileLd * 4;
+static constexpr int kAsyncStagingBytes = kEpiWarps * 4096;
+static constexpr int kAsyncVecBytes = 2 * kTileN * 4;  // vec0 and vec1 of the tile's 128 columns, [chunk][vec0 32 | vec1 32]
+static constexpr int kAsyncSmemBytes =
+    kStages * kStageBytes + kAsyncStagingBytes + kTileBufBytes + kAsyncVecBytes + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(kAsyncSmemBytes <= 227 * 1024, "shared memory per block");
+__host__ __device__ constexpr int km_smem_bytes(int epi) { return km_async(epi) ? kAsyncSmemBytes : kSmemBytes; }
+
+struct KmSmem : SmemLayout {
+  float* tile = nullptr;  // [kTileM][kTileLd]: the accumulator of one tile (async epilogue only)
+  uint64_t* tile_full = nullptr;
+  uint64_t* tile_empty = nullptr;
+  int* tile_id = nullptr;  // id of the tile in the buffer (-1: no more tiles)
+};
+template <bool ASYNC>
+__device__ __forceinline__ KmSmem carve_km_smem(uint8_t* smem_raw) {
+  KmSmem L;
+  if (!ASYNC) {
+    static_cast<SmemLayout&>(L) = carve_smem(smem_raw);
+    return L;
+  }
+  L.stages = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  L.staging = L.stages + kStages * kStageBytes;
+  L.tile = reinterpret_cast<float*>(L.staging + kAsyncStagingBytes);
+  L.raw = nullptr;
+  L.vec = L.tile + kTileM * kTileLd;
+  L.full_bar = reinterpret_cast<uint64_t*>(L.vec + kAsyncVecBytes / 4);
+  L.empty_bar = L.full_bar + kStages;
+  L.ring_bar = L.empty_bar + kStages;
+  L.tile_full = L.ring_bar + 8;
+  L.tile_empty = L.tile_full + 1;
+  L.tile_ring = reinterpret_cast<int*>(L.tile_empty + 1);
+  L.tile_id = L.tile_ring + 8;
+  return L;
+}
+
 // Accumulator of one warpgroup (m64n128 wgmma layout: register 4j + e of thread (warp w, lane l) is row 16w + l/4 + 8(e/2),
 // column 8j + 2(l%4) + e%2) -> columns [64 slab, +64) of the warpgroup's transpose buffer.
 __device__ __forceinline__ void wgmma_acc_to_raw(const float (&acc)[64], float* raw, int slab, int w, int lane) {
@@ -74,6 +124,22 @@ __device__ __forceinline__ void wgmma_acc_to_raw(const float (&acc)[64], float* 
       const int c = 8 * jj + 2 * (lane & 3) + (e & 1);
       raw[r * kRawLd + c] = acc[4 * (8 * slab + jj) + e];
     }
+}
+// Shared-memory accesses of the whole-tile buffer by 32-bit address: through a generic pointer the compiler keeps one 64-bit
+// address per element live and runs out of the 128 registers a 512-thread CTA allows.
+__device__ __forceinline__ void sts_f32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v)); }
+__device__ __forceinline__ float lds_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+  return v;
+}
+// The same transpose for all 128 columns at once: warpgroup g's accumulator -> rows [64 g, +64) of the whole-tile buffer.
+__device__ __forceinline__ void wgmma_acc_to_tile(const float (&acc)[64], uint32_t tile, int g, int w, int lane) {
+  const uint32_t base = tile + 4 * ((64 * g + 16 * w + (lane >> 2)) * kTileLd + 2 * (lane & 3));
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) sts_f32(base + 4 * ((8 * (e >> 1)) * kTileLd + 8 * j + (e & 1)), acc[4 * j + e]);
 }
 
 // Epilogue walk shared by both kernels.  For each 64-column slab the warpgroup's accumulator goes through the transpose
@@ -523,10 +589,19 @@ __device__ __forceinline__ void km_chunk(const KmParams& p, const CUtensorMap* t
     // column sums of the chunk straight from the staged copy: lane c adds column c over the 32 rows
     float cs = 0.f;
     if (OUT16 == 2) {
+      // p.colsumsq: the exact Gram diagonal, sum of (hi + lo)^2 in fp64 (two partial sums: half the dependent DFMA chain)
+      double sq[2] = {0.0, 0.0};
 #pragma unroll
-      for (int r = 0; r < 32; ++r)
-        cs += __half2float(*reinterpret_cast<const __half*>(buf + r * 64 + lane * 2)) +
-              __half2float(*reinterpret_cast<const __half*>(buf + 2048 + r * 64 + lane * 2));
+      for (int r = 0; r < 32; ++r) {
+        const float h = __half2float(*reinterpret_cast<const __half*>(buf + r * 64 + lane * 2));
+        const float l = __half2float(*reinterpret_cast<const __half*>(buf + 2048 + r * 64 + lane * 2));
+        cs += h + l;
+        if (p.colsumsq != nullptr) {
+          const double v = static_cast<double>(h) + static_cast<double>(l);
+          sq[r & 1] = fma(v, v, sq[r & 1]);
+        }
+      }
+      if (p.colsumsq != nullptr && col0 + lane < p.N) atomicAdd(p.colsumsq + col0 + lane, sq[0] + sq[1]);
     } else if (OUT16 == 1) {
 #pragma unroll
       for (int r = 0; r < 32; ++r) cs += __half2float(*reinterpret_cast<const __half*>(buf + r * 64 + lane * 2));
@@ -548,17 +623,20 @@ __device__ __forceinline__ void km_chunk(const KmParams& p, const CUtensorMap* t
 // SPLIT (fp16 pairs): a stage holds A_hi, A_lo, B_hi, B_lo with 32 K-elements each (64 B rows, 64 B swizzle, 8 KB per tile);
 // A_hi B_hi^T accumulates on its own, A_lo B_hi^T + A_hi B_lo^T in a second accumulator, and their fp32 sum goes through the
 // epilogue once.
+// Slab producers (km_async): 512 threads, warpgroup 3 runs the epilogue (see KmSmem).
 template <int EPI, bool F16, int OUT16, bool SPLIT>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(km_threads(EPI), 1)
 gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmOut2,
                    const __grid_constant__ CUtensorMap tmAlo, const __grid_constant__ CUtensorMap tmBlo, KmParams p) {
   static_assert(!SPLIT || F16, "split operands are fp16 pairs");
+  constexpr bool ASYNC = km_async(EPI);
+  static_assert(!(ASYNC && SPLIT), "the split update keeps its in-place epilogue");
   constexpr int ROW_BYTES = SPLIT ? 64 : 128;     // one swizzle row of K
   constexpr int BK = ROW_BYTES / (F16 ? 2 : 4);   // K elements per stage
   constexpr int A_BYTES = kTileM * ROW_BYTES;
   extern __shared__ uint8_t smem_raw[];
-  const SmemLayout L = carve_smem(smem_raw);
+  const KmSmem L = carve_km_smem<ASYNC>(smem_raw);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -581,6 +659,10 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       mbar_init(&L.empty_bar[s], 8);  // one arrive per consumer warp
     }
     for (int r = 0; r < 8; ++r) mbar_init(&L.ring_bar[r], 1);
+    if (ASYNC) {
+      mbar_init(L.tile_full, 256);   // every MMA thread, after its part of the accumulator
+      mbar_init(L.tile_empty, 32 * kEpiWarps);  // every epilogue thread, after its last read of the buffer
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -589,6 +671,47 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   // persistent and shares the GPU with the factor / solve chains' kernels) simply takes fewer tiles instead of stretching the
   // whole launch by its late start.  Without a counter the tiles are strided statically.  Either way the producer publishes
   // every tile id (then -1) in an 8-slot ring; the stage ring keeps it within ~kStages tiles of the consumers, so slots are free.
+  if (ASYNC && ((warp >= 1 && warp < 4) || warp >= 12)) {
+    // epilogue warp e (warps 1-3 -> 0-2, warps 12-16 -> 3-7): rows [32 (e % 4), +32) and chunks 2 (e / 4), 2 (e / 4) + 1 of each tile
+    const int e = warp < 4 ? warp - 1 : warp - 9;
+    const int rb = e & 3, cb = 2 * (e >> 2);
+    uint8_t* sbuf = L.staging + e * 4096;
+    const float ascale = p.acc_scale_ptr ? __ldg(p.acc_scale_ptr) * p.acc_scale : p.acc_scale;
+    uint32_t staged = 0;  // chunks this warp has stored: single fp16 outputs alternate the two halves of sbuf
+    for (uint32_t tl = 0;; ++tl) {
+      mbar_wait(L.tile_full, tl & 1);
+      const int t = *L.tile_id;
+      if (t < 0) break;
+      const int m0 = (t / n_tiles) * kTileM;
+      const int n0 = (t % n_tiles) * kTileN;
+      {  // the tile's vec0 / vec1 columns, once for all epilogue warps (after all of them are done with the previous tile's)
+        named_bar_sync(1, 32 * kEpiWarps);
+        const int te = 32 * e + lane, which = te >> 7, c = (te >> 5) & 3;
+        const float* v = which ? p.vec1 : p.vec0;
+        const int n = n0 + 32 * c + lane;
+        L.vec[64 * c + 32 * which + lane] = (v && n < p.N) ? __ldg(v + n) : 0.f;
+        named_bar_sync(1, 32 * kEpiWarps);
+      }
+      const uint32_t src = smem_u32(L.tile + (32 * rb + lane) * kTileLd);
+#pragma unroll 1
+      for (int k = 0; k < 2; ++k) {
+        const int c = cb + k;
+        const int col0 = n0 + 32 * c;
+        if (col0 >= p.N) {  // warp-uniform; columns only run out in the last chunks of a tile
+          if (k == 1) mbar_arrive(L.tile_empty);
+          continue;
+        }
+        float o[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[i] = lds_f32(src + 4 * (32 * c + i));
+        if (k == 1) mbar_arrive(L.tile_empty);  // the MMA warpgroups may dump the next tile
+        km_chunk<EPI, OUT16>(p, &tmOut, &tmOut2, o, L.vec + 64 * c, sbuf, staged & 1, m0 + 32 * rb, col0, lane, ascale);
+        ++staged;
+      }
+    }
+    if (lane == 0) bulk_wait0();
+    return;
+  }
   if (wg == 0) {
     if (warp == 0 && elect_one()) {
       uint32_t it = 0, tl = 0;
@@ -632,6 +755,12 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   for (uint32_t tl = 0;; ++tl) {
     mbar_wait(&L.ring_bar[tl & 7], (tl >> 3) & 1);
     const int t = L.tile_ring[tl & 7];
+    if (ASYNC && t < 0) {  // no more tiles: tell the epilogue warpgroup once it has read the last one
+      mbar_wait(L.tile_empty, (tl & 1) ^ 1);
+      if (threadIdx.x == 128) *L.tile_id = -1;
+      mbar_arrive(L.tile_full);
+      return;
+    }
     if (t < 0) break;
     const int m0 = (t / n_tiles) * kTileM;
     const int n0 = (t % n_tiles) * kTileN;
@@ -704,6 +833,13 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
     }
 
+    if (ASYNC) {
+      mbar_wait(L.tile_empty, (tl & 1) ^ 1);  // the epilogue warpgroup has read the previous tile
+      wgmma_acc_to_tile(acc, smem_u32(L.tile), g, w, lane);
+      if (threadIdx.x == 128) *L.tile_id = t;
+      mbar_arrive(L.tile_full);
+      continue;
+    }
     auto to_raw = [&](float* rw, int slab) { wgmma_acc_to_raw(acc, rw, slab, w, lane); };
     auto chunk_fn = [&](float (&o)[32], int slab, int r_off, int c_off) {
       const int col0 = n0 + c_off;
@@ -764,9 +900,9 @@ int make_tmap_any(CUtensorMap* out, const void* base, int64_t rows, int64_t cols
 
 // The kernels of one family share a signature, so the "attribute set" flag lives in each launcher instantiation.
 template <typename K>
-static cudaError_t set_smem_attr_once(K kern, bool& done) {
+static cudaError_t set_smem_attr_once(K kern, bool& done, int bytes = kSmemBytes) {
   if (!done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     if (e != cudaSuccess) return e;
     done = true;
   }
@@ -797,14 +933,14 @@ template <int EPI, bool F16, int OUT16, bool SPLIT = false>
 static cudaError_t launch_km_t(const KmLaunch& k, cudaStream_t st) {
   auto kern = gemm_kmajor_kernel<EPI, F16, OUT16, SPLIT>;
   static bool attr_done = false;
-  cudaError_t e = set_smem_attr_once(kern, attr_done);
+  cudaError_t e = set_smem_attr_once(kern, attr_done, km_smem_bytes(EPI));
   if (e != cudaSuccess) return e;
   const int m_tiles = (k.p.M + kTileM - 1) / kTileM;
   const int n_tiles = (k.p.N + kTileN - 1) / kTileN;
   const long long total = static_cast<long long>(m_tiles) * n_tiles;
   if (total == 0) return cudaSuccess;
   const unsigned grid = static_cast<unsigned>(total < k.num_sms ? total : k.num_sms);
-  kern<<<grid, kThreads, kSmemBytes, st>>>(k.tmA, k.tmB, k.tmOut, OUT16 == 2 ? k.tmOut2 : k.tmOut, SPLIT ? k.tmAlo : k.tmA,
+  kern<<<grid, km_threads(EPI), km_smem_bytes(EPI), st>>>(k.tmA, k.tmB, k.tmOut, OUT16 == 2 ? k.tmOut2 : k.tmOut, SPLIT ? k.tmAlo : k.tmA,
                                            SPLIT ? k.tmBlo : k.tmB, k.p);
   return cudaGetLastError();
 }
