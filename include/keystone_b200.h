@@ -159,6 +159,47 @@ KS_API int32_t ks_gmm_posteriors(int64_t ctx, int64_t gmm, int64_t x, int64_t* o
 KS_API int32_t ks_fisher_vector_apply(int64_t ctx, int64_t gmm, int64_t descriptors, const int64_t* item_offsets, int64_t n_items,
                                       int64_t* out_m);
 
+/* ---- Gaussian-mixture EM and k-means++ (DESIGN.md section 17) ---------------------------------------------------------------
+ * The fits of K/nodes/learning/{GaussianMixtureModelEstimator,KMeansPlusPlus}.scala on the rows of x (N x dim), in fp64 on the
+ * device, without float atomics (a repeated fit returns identical bits).  Not collective: each rank fits on the rows it is given.
+ * Every fit writes ks_last_fit_stats_json: solver ("gmm" / "kmeans"), n, d, k, iterations, stop_reason ("max_iterations", "cost",
+ * "min_cluster_size"), cost_history, seed_rows, seeding / init / estep / stats / mstep milliseconds and launches.
+ * Rejected with KS_ERR_INVALID: k <= 0, N < k, dim > 1024, non-finite input, uniforms outside [0, 1), and fewer distinct points than
+ * centres; a cluster the k-means passes leave empty is an error that names it (the reference divides by zero there).
+ *
+ * Randomness: the reference's MersenneTwister / Multinomial stream is not reproduced; the caller passes the uniforms.  k-means++
+ * takes num_means uniforms u_j in [0, 1):
+ *   centre 0 is row min(floor(u_0 N), N - 1);
+ *   after centre j - 1, every row holds d_n = min over the centres so far of 1/2 sum_d (x_nd - c_d)^2 (fp64, the sum over d in
+ *   order, no fused multiply-add).  Blocks are the rows [256 b, 256 b + 256); B_b = the tree sum of the block's d (pairs at
+ *   distance 128, 64, ..., 1, zeros past N); P_b = B_0 + ... + B_(b-1) and W = P_nblocks, summed left to right.  W = 0: error.
+ *   Centre j is in the first block with P_b + B_b > u_j W (none: the last block with B_b > 0), at the first row n of that block with
+ *   P_b + s_n > u_j W, s_n the inclusive prefix sum of d over the block's rows in order (none: the block's last row with d_n > 0). */
+/* KMeansPlusPlusEstimator(num_means, max_iterations, stop_tolerance).fit(x): the seeding above, then up to max_iterations Lloyd
+ * passes (assignment to the first nearest centre, cost = mean best distance, means = sums / counts; stop after the pass whose
+ * cost fails (prev - cur) >= stop_tolerance |prev|).  means_out: num_means x dim row-major; seed_rows_or_null: the num_means
+ * seed rows. */
+KS_API int32_t ks_kmeans_fit(int64_t ctx, int64_t x, int64_t num_means, int32_t max_iterations, double stop_tolerance,
+                             const double* uniforms, double* means_out, int64_t* seed_rows_or_null, int32_t* iterations_or_null);
+/* KMeansModel(means).apply(x): the N x num_means one-hot assignment (fp32) to the first nearest of the means (num_means x dim,
+ * row-major). */
+KS_API int32_t ks_kmeans_assign(int64_t ctx, int64_t x, const double* means_rowmajor, int64_t num_means, int64_t dim, int64_t* out_m);
+/* GaussianMixtureModelEstimator(k, maxIterations, minClusterSize, stopTolerance, weightThreshold, smallVarianceThreshold,
+ * absoluteVarianceThreshold, initializationMethod).fit(x).  initialization 0: k-means++ (uniforms: k values, the rule above; one
+ * Lloyd pass, then weights, means and variances of the hard assignment to the updated means); 1: random (uniforms: k x dim
+ * row-major, means = colMin + u range, variances = 0.1 range^2, weights 1/k).  Variances are floored at
+ * max(smallVarianceThreshold varGlobal_d, absoluteVarianceThreshold).  EM stops when (cur - prev) < stopTolerance |prev| (from the
+ * second iteration; that E-step counts as an iteration, no M-step follows), or when a component's posterior mass is below
+ * minClusterSize (the previous parameters are kept).  weightThreshold must lie in [0, 1/k); absoluteVarianceThreshold must be > 0.
+ * Returns a model handle with weightThreshold 1e-4 (as the reference's GaussianMixtureModel(means, vars, weights)), its means and
+ * variances (dim x k column-major), k weights and the number of E-steps evaluated. */
+KS_API int32_t ks_gmm_fit(int64_t ctx, int64_t x, int64_t k, int32_t max_iterations, double min_cluster_size, double stop_tolerance,
+                          double weight_threshold, double small_variance_threshold, double absolute_variance_threshold,
+                          int32_t initialization, const double* uniforms, int64_t* out_gmm, double* means_colmajor_out,
+                          double* variances_colmajor_out, double* weights_out, int32_t* iterations_or_null);
+/* out = rows rows[0..n) of m, in that order, as a new matrix (ColumnSampler on an item batch); indices must lie in [0, rows). */
+KS_API int32_t ks_matrix_gather_rows(int64_t ctx, int64_t m, const int64_t* rows, int64_t n, int64_t* out_m);
+
 /* ---- Convolver [andThen SymmetricRectifier andThen Pooler(sum) andThen ImageVectorizer] ---------------------------------
  * The featurizer of K/pipelines/images/cifar/RandomPatchCifar.scala:59-63 (K/nodes/images/Convolver.scala:20-203,
  * SymmetricRectifier.scala:7-32, Pooler.scala:21-69, K/utils/Stats.scala:112-123).  filters: DenseMatrix (n_filters x

@@ -218,6 +218,49 @@ JFN(jlong, fisherVectorApply)(JNIEnv* env, jobject, jlong ctx, jlong gmm, jlong 
   const int32_t rc = ks_fisher_vector_apply(ctx, gmm, descriptors, o.data(), o.n - 1, &h);
   return ok(env, ctx, rc) ? h : 0;
 }
+// ---- GMM EM, k-means++, row gather (not collective; DESIGN.md section 17).  uniforms: the draw rule of the header.
+// means / variances out: D x K DenseMatrix.data (column-major); returns the model handle
+JFN(jlong, gmmFit)(JNIEnv* env, jobject, jlong ctx, jlong x, jlong k, jint maxIterations, jdouble minClusterSize, jdouble stopTolerance,
+                   jdouble weightThreshold, jdouble smallVarianceThreshold, jdouble absoluteVarianceThreshold, jint initialization,
+                   jdoubleArray uniforms, jdoubleArray meansOut, jdoubleArray variancesOut, jdoubleArray weightsOut) {
+  int64_t h = 0;
+  jdouble* u = env->GetDoubleArrayElements(uniforms, nullptr);
+  jdouble* mu = env->GetDoubleArrayElements(meansOut, nullptr);
+  jdouble* var = env->GetDoubleArrayElements(variancesOut, nullptr);
+  jdouble* w = env->GetDoubleArrayElements(weightsOut, nullptr);
+  const int32_t rc = (u && mu && var && w) ? ks_gmm_fit(ctx, x, k, maxIterations, minClusterSize, stopTolerance, weightThreshold,
+                                                        smallVarianceThreshold, absoluteVarianceThreshold, initialization, u, &h, mu,
+                                                        var, w, nullptr)
+                                           : KS_ERR_INVALID;
+  if (w) env->ReleaseDoubleArrayElements(weightsOut, w, 0);
+  if (var) env->ReleaseDoubleArrayElements(variancesOut, var, 0);
+  if (mu) env->ReleaseDoubleArrayElements(meansOut, mu, 0);
+  if (u) env->ReleaseDoubleArrayElements(uniforms, u, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+// meansOut: numMeans x dim row-major; returns the number of Lloyd passes
+JFN(jint, kmeansFit)(JNIEnv* env, jobject, jlong ctx, jlong x, jlong numMeans, jint maxIterations, jdouble stopTolerance,
+                     jdoubleArray uniforms, jdoubleArray meansOut) {
+  int32_t it = 0;
+  jdouble* u = env->GetDoubleArrayElements(uniforms, nullptr);
+  jdouble* mu = env->GetDoubleArrayElements(meansOut, nullptr);
+  const int32_t rc = (u && mu) ? ks_kmeans_fit(ctx, x, numMeans, maxIterations, stopTolerance, u, mu, nullptr, &it) : KS_ERR_INVALID;
+  if (mu) env->ReleaseDoubleArrayElements(meansOut, mu, 0);
+  if (u) env->ReleaseDoubleArrayElements(uniforms, u, JNI_ABORT);
+  return ok(env, ctx, rc) ? it : 0;
+}
+JFN(jlong, kmeansAssign)(JNIEnv* env, jobject, jlong ctx, jlong x, jdoubleArray meansRowMajor, jlong numMeans, jlong dim) {
+  int64_t h = 0;
+  jdouble* mu = env->GetDoubleArrayElements(meansRowMajor, nullptr);
+  const int32_t rc = mu ? ks_kmeans_assign(ctx, x, mu, numMeans, dim, &h) : KS_ERR_INVALID;
+  if (mu) env->ReleaseDoubleArrayElements(meansRowMajor, mu, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, matrixGatherRows)(JNIEnv* env, jobject, jlong ctx, jlong m, jlongArray rows) {
+  int64_t h = 0;
+  LongArray r(env, rows);
+  return ok(env, ctx, ks_matrix_gather_rows(ctx, m, r.data(), r.n, &h)) ? h : 0;
+}
 JFN(jlong, matrixNormalizeRows)(JNIEnv* env, jobject, jlong ctx, jlong m) {
   int64_t h = 0;
   return ok(env, ctx, ks_matrix_normalize_rows(ctx, m, &h)) ? h : 0;

@@ -2122,6 +2122,51 @@ KS_API int32_t ks_matrix_normalize_rows(int64_t ctx, int64_t m, int64_t* out_m) 
   });
 }
 
+// ---------------------------------------------------------------- GMM EM, k-means++, row gather (gmm_fit.cu)
+KS_API int32_t ks_kmeans_fit(int64_t ctx, int64_t x, int64_t num_means, int32_t max_iterations, double stop_tolerance,
+                             const double* uniforms, double* means_out, int64_t* seed_rows_or_null, int32_t* iterations_or_null) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!means_out) throw KsError{KS_ERR_INVALID, "null means_out"};
+    const KmeansResult r = kmeans_fit(c, c.matrix(x), num_means, max_iterations, stop_tolerance, uniforms);
+    std::copy(r.means.begin(), r.means.end(), means_out);
+    if (seed_rows_or_null) std::copy(r.seeds.begin(), r.seeds.end(), seed_rows_or_null);
+    if (iterations_or_null) *iterations_or_null = r.iterations;
+  });
+}
+KS_API int32_t ks_kmeans_assign(int64_t ctx, int64_t x, const double* means_rowmajor, int64_t num_means, int64_t dim, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(kmeans_assign(c, c.matrix(x), means_rowmajor, num_means, dim));
+  });
+}
+KS_API int32_t ks_gmm_fit(int64_t ctx, int64_t x, int64_t k, int32_t max_iterations, double min_cluster_size, double stop_tolerance,
+                          double weight_threshold, double small_variance_threshold, double absolute_variance_threshold,
+                          int32_t initialization, const double* uniforms, int64_t* out_gmm, double* means_colmajor_out,
+                          double* variances_colmajor_out, double* weights_out, int32_t* iterations_or_null) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_gmm) throw KsError{KS_ERR_INVALID, "null out_gmm"};
+    GmmFitArgs a;
+    a.k = k;
+    a.max_iter = max_iterations;
+    a.min_cluster = min_cluster_size;
+    a.tol = stop_tolerance;
+    a.thr = weight_threshold;
+    a.small_var = small_variance_threshold;
+    a.abs_var = absolute_variance_threshold;
+    a.init = initialization;
+    a.uniforms = uniforms;
+    int it = 0;
+    *out_gmm = gmm_fit(c, c.matrix(x), a, means_colmajor_out, variances_colmajor_out, weights_out, &it);
+    if (iterations_or_null) *iterations_or_null = it;
+  });
+}
+KS_API int32_t ks_matrix_gather_rows(int64_t ctx, int64_t m, const int64_t* rows, int64_t n, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(gather_rows(c, c.matrix(m), rows, n));
+  });
+}
+
 // ---------------------------------------------------------------- models
 KS_API int32_t ks_model_from_host(int64_t ctx, const double* const* xs, const int64_t* block_rows, int32_t n_blocks, int64_t k,
                            const double* b_or_null, const double* const* means_or_null, int32_t block_size, int64_t* out_model) {

@@ -390,5 +390,33 @@ std::unique_ptr<Matrix> gmm_posteriors(Ctx& c, const Gmm& g, Matrix& X);
 std::unique_ptr<Matrix> fisher_vector_apply(Ctx& c, const Gmm& g, Matrix& X, const int64_t* item_offsets, int64_t n_items);
 std::unique_ptr<Matrix> normalize_rows(Ctx& c, Matrix& in);
 void launch_signed_sqrt(Ctx& c, const float* in, float* out, int64_t n);
+// building blocks of the mixture fit (fisher.cu): the posterior kernel with epilogue epi (1: posteriors and the per-row Xerox
+// log-sum-exp into row_out, 2: one-hot hard assignment and the best distance into row_out; Q: rows x g.k, row_out indexed from row 0
+// of X), fv_stats_kernel over n_items row ranges d_offs (device, absolute rows of X; Q row 0 is row q_row0), its tiles per item, and
+// the rows of one posterior chunk (256 MB of fp64 Q)
+void launch_gmm_estep(Ctx& c, const Gmm& g, const Matrix& X, int64_t row0, int64_t rows, double* Q, float* out, int64_t ldo, int epi,
+                      double* row_out);
+void launch_fv_stats(Ctx& c, const Matrix& X, const double* Q, int64_t ldq, int64_t q_row0, const int64_t* d_offs, int64_t n_items, int D,
+                     int K, double* S);
+int64_t fv_stats_tiles(int D, int K);
+int64_t posterior_chunk_rows(const Gmm& g);
+
+// Gaussian-mixture EM and k-means++ (gmm_fit.cu); not collective.  uniforms: the draw rule of include/keystone_b200.h.
+struct KmeansResult {
+  std::vector<double> means;  // K x D row-major
+  std::vector<int64_t> seeds;
+  int iterations = 0;
+};
+KmeansResult kmeans_fit(Ctx& c, Matrix& X, int64_t k, int max_iter, double tol, const double* uniforms);
+std::unique_ptr<Matrix> kmeans_assign(Ctx& c, Matrix& X, const double* means_rowmajor, int64_t k, int64_t dim);
+struct GmmFitArgs {
+  int64_t k = 0;
+  int max_iter = 100, init = 0;
+  double min_cluster = 40, tol = 1e-4, thr = 1e-4, small_var = 1e-2, abs_var = 1e-9;
+  const double* uniforms = nullptr;
+};
+// returns the model handle (weightThreshold 1e-4); means / vars D x K column-major, weights K
+int64_t gmm_fit(Ctx& c, Matrix& X, const GmmFitArgs& a, double* means_colmajor, double* vars_colmajor, double* weights, int* iterations);
+std::unique_ptr<Matrix> gather_rows(Ctx& c, Matrix& X, const int64_t* rows, int64_t n);
 
 }  // namespace ks

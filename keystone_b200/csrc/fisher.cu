@@ -68,13 +68,22 @@ __global__ void lcs_gather_kernel(const float2* __restrict__ stats, int64_t n_im
 static constexpr int kGR = 32;        // rows per CTA (one per lane)
 static constexpr int kGThreads = 256; // 8 warps: warp w owns components k0 + w + 8 j, j < 4, of each 32-component chunk
 static constexpr int kGSLd = kGR + 1;
+static constexpr int kEpiPosterior = 0, kEpiPosteriorLse = 1, kEpiAssign = 2;
 
 // Q[row][k] (fp64, ldq) and / or out (fp32, ldo) = thresholded, renormalised posteriors of rows [32 blockIdx.x, +32) of X (N x D).
 // mu / hiv: [d][k] = mean, 0.5 / variance; ck[k] = log w_k - 1/2 sum_d log var_dk - D/2 log 2 pi.
+// The epilogue is a compile-time choice (one kernel, so the three share the load phase and the log-likelihood loop exactly):
+//   kEpiPosterior     the posteriors (GaussianMixtureModel.apply, FisherVector);
+//   kEpiPosteriorLse  the same, and first row_out[row] = the reference's incremental ("Xerox") log-sum-exp of the row's raw
+//                     log-likelihoods, one lane per row over k in order (GaussianMixtureModelEstimator.scala:127-148);
+//   kEpiAssign        hard assignment: Q row (and out) = one-hot at the first argmax of the log-likelihood, row_out[row] = -max.  With
+//                     hiv = 1/2 and ck = 0 that is the first argmin of 1/2 |x - c|^2 and the distance itself (KMeansModel.apply).
+template <int kEpi>
 __global__ void __launch_bounds__(kGThreads) gmm_posterior_kernel(const float* __restrict__ X, int64_t ldx, int64_t rows, int D, int K,
                                                                   const double* __restrict__ mu, const double* __restrict__ hiv,
                                                                   const double* __restrict__ ck, double thr, double* __restrict__ Q,
-                                                                  int64_t ldq, float* __restrict__ out, int64_t ldo) {
+                                                                  int64_t ldq, float* __restrict__ out, int64_t ldo,
+                                                                  double* __restrict__ row_out) {
   extern __shared__ float sx[];  // [D][kGSLd]: this CTA's rows, transposed
   __shared__ double smu[32][32], shv[32][32];
   const int64_t r0 = static_cast<int64_t>(blockIdx.x) * kGR;
@@ -113,6 +122,48 @@ __global__ void __launch_bounds__(kGThreads) gmm_posterior_kernel(const float* _
       }
   }
   __syncthreads();  // the log-likelihoods of the CTA's rows are in Q
+  if constexpr (kEpi == kEpiAssign) {
+    for (int r = warp; r < nr; r += kGThreads / 32) {
+      double* q = Q + (r0 + r) * ldq;
+      double m = -INFINITY;
+      int best = K;
+      for (int k = lane; k < K; k += 32)
+        if (q[k] > m) {  // strict: the first of equal values within the lane
+          m = q[k];
+          best = k;
+        }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const double om = __shfl_xor_sync(0xffffffffu, m, o);
+        const int ob = __shfl_xor_sync(0xffffffffu, best, o);
+        if (om > m || (om == m && ob < best)) {
+          m = om;
+          best = ob;
+        }
+      }
+      for (int k = lane; k < K; k += 32) {
+        q[k] = k == best ? 1.0 : 0.0;
+        if (out) out[(r0 + r) * ldo + k] = k == best ? 1.f : 0.f;
+      }
+      if (lane == 0) row_out[r0 + r] = -m;
+    }
+    return;
+  }
+  if constexpr (kEpi == kEpiPosteriorLse) {
+    if (threadIdx.x < nr) {
+      const double* q = Q + (r0 + threadIdx.x) * ldq;
+      double lse = q[0];
+      for (int k = 1; k < K; ++k) {
+        const double l = q[k], delta = lse - l;
+        double inc = 0.0;  // delta <= -30 adds no weight
+        if (delta > 30.0) inc = delta;
+        else if (delta > -30.0) inc = log(exp(delta) + 1.0);
+        lse = inc + l;
+      }
+      row_out[r0 + threadIdx.x] = lse;
+    }
+    __syncthreads();  // the raw log-likelihoods are read before the exp pass overwrites them
+  }
   for (int r = warp; r < nr; r += kGThreads / 32) {
     double* q = Q + (r0 + r) * ldq;
     double m = -INFINITY;
@@ -385,22 +436,45 @@ int64_t gmm_create(Ctx& c, const double* means, const double* vars, const double
   return id;
 }
 
-// posteriors of rows [row0, row0 + rows) of X into Q (fp64, ldq) and / or out (fp32)
-static void launch_posteriors(Ctx& c, const Gmm& g, const Matrix& X, int64_t row0, int64_t rows, double* Q, int64_t ldq, float* out,
-                              int64_t ldo) {
+template <int kEpi>
+static void launch_posterior_epi(Ctx& c, const Gmm& g, const Matrix& X, int64_t row0, int64_t rows, double* Q, int64_t ldq, float* out,
+                                 int64_t ldo, double* row_out) {
   if (rows == 0) return;
   const int64_t blocks = (rows + kGR - 1) / kGR;
   if (blocks > 0x7fffffffLL) throw KsError{KS_ERR_INVALID, "GaussianMixtureModel: too many rows"};
   const size_t smem = sizeof(float) * static_cast<size_t>(g.dim) * kGSLd;
-  KS_CUDA(cudaFuncSetAttribute(gmm_posterior_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  gmm_posterior_kernel<<<static_cast<unsigned>(blocks), kGThreads, smem, c.st>>>(X.d + row0 * X.ld, X.ld, rows, static_cast<int>(g.dim),
-                                                                                  static_cast<int>(g.k), g.mu(), g.hiv(), g.ck(), g.thr, Q, ldq,
-                                                                                  out, ldo);
+  KS_CUDA(cudaFuncSetAttribute(gmm_posterior_kernel<kEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  gmm_posterior_kernel<kEpi><<<static_cast<unsigned>(blocks), kGThreads, smem, c.st>>>(
+      X.d + row0 * X.ld, X.ld, rows, static_cast<int>(g.dim), static_cast<int>(g.k), g.mu(), g.hiv(), g.ck(), g.thr, Q, ldq, out, ldo,
+      row_out ? row_out + row0 : nullptr);
   c.launches += 1;
 }
 
+// posteriors of rows [row0, row0 + rows) of X into Q (fp64, ldq) and / or out (fp32)
+static void launch_posteriors(Ctx& c, const Gmm& g, const Matrix& X, int64_t row0, int64_t rows, double* Q, int64_t ldq, float* out,
+                              int64_t ldo) {
+  launch_posterior_epi<kEpiPosterior>(c, g, X, row0, rows, Q, ldq, out, ldo, nullptr);
+}
+
+void launch_gmm_estep(Ctx& c, const Gmm& g, const Matrix& X, int64_t row0, int64_t rows, double* Q, float* out, int64_t ldo, int epi,
+                      double* row_out) {
+  if (epi == kEpiPosteriorLse) launch_posterior_epi<kEpiPosteriorLse>(c, g, X, row0, rows, Q, g.k, out, ldo, row_out);
+  else if (epi == kEpiAssign) launch_posterior_epi<kEpiAssign>(c, g, X, row0, rows, Q, g.k, out, ldo, row_out);
+  else throw KsError{KS_ERR_INVALID, "launch_gmm_estep: unknown epilogue"};
+}
+
+void launch_fv_stats(Ctx& c, const Matrix& X, const double* Q, int64_t ldq, int64_t q_row0, const int64_t* d_offs, int64_t n_items, int D,
+                     int K, double* S) {
+  const int m = 2 * D + 1;
+  const unsigned tiles = static_cast<unsigned>(((m + kFT - 1) / kFT) * ((K + kFT - 1) / kFT));
+  fv_stats_kernel<<<dim3(tiles, static_cast<unsigned>(n_items)), kFThreads, 0, c.st>>>(X.d, X.ld, Q, ldq, q_row0, d_offs, D, K, S);
+  c.launches += 1;
+}
+
+int64_t fv_stats_tiles(int D, int K) { return static_cast<int64_t>((2 * D + 1 + kFT - 1) / kFT) * ((K + kFT - 1) / kFT); }
+
 // the fp64 posterior scratch of one launch is bounded to 256 MB of rows
-static int64_t posterior_chunk_rows(const Gmm& g) { return std::max<int64_t>(kGR, ((int64_t(256) << 20) / (8 * g.k)) / kGR * kGR); }
+int64_t posterior_chunk_rows(const Gmm& g) { return std::max<int64_t>(kGR, ((int64_t(256) << 20) / (8 * g.k)) / kGR * kGR); }
 
 std::unique_ptr<Matrix> gmm_posteriors(Ctx& c, const Gmm& g, Matrix& X) {
   if (X.cols != g.dim) throw KsError{KS_ERR_INVALID, "GaussianMixtureModel.apply: input columns != model dimension"};

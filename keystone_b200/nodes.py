@@ -1375,3 +1375,165 @@ class SignedHellingerMapper(Transformer):
 
 class BatchSignedHellingerMapper(SignedHellingerMapper):
     """BatchSignedHellingerMapper: the same map on (dim x n) Float items (an ``ItemBatch`` keeps its offsets)."""
+
+
+# ------------------------------------------------------------------------------------------ mixture and k-means fits
+# GaussianMixtureModelEstimator, KMeansPlusPlusEstimator / KMeansModel, (Scala)GMMFisherVectorEstimator, ColumnSampler
+# (K/nodes/learning/{GaussianMixtureModelEstimator,KMeansPlusPlus}.scala, K/nodes/images/FisherVector.scala:55-95,
+# K/nodes/stats/Sampling.scala).  DESIGN.md section 17.
+def _fit_rows(ctx: Optional[Context], data) -> DeviceMatrix:
+    """The sample rows of a fit: an ``ItemBatch`` (every descriptor is a sample), a device matrix or host rows."""
+    if isinstance(data, ItemBatch):
+        return data.matrix
+    return _device_matrix(ctx, data)
+
+
+class KMeansModel(Transformer):
+    """``KMeansModel(means)`` (KMeansPlusPlus.scala:16-70), means numMeans x dim: ``apply`` returns the one-hot assignment to the first
+    nearest mean (a vector for a vector, an N x numMeans device batch for a batch)."""
+
+    def __init__(self, means, ctx: Optional[Context] = None):
+        self.means = np.ascontiguousarray(np.atleast_2d(np.asarray(means, dtype=np.float64)))
+        self.ctx = ctx
+
+    def apply(self, data):
+        single = isinstance(data, np.ndarray) and data.ndim == 1
+        x = _device_matrix(self.ctx, data)
+        h = C.c_int64(0)
+        k, d = self.means.shape
+        check(x.ctx.handle, lib().ks_kmeans_assign(x.ctx.handle, x.handle, self.means.ctypes.data_as(C.c_void_p), k, d, C.byref(h)))
+        out = DeviceMatrix(x.ctx, h.value, x.rows, k)
+        return out.to_numpy()[0] if single else out
+
+
+class KMeansPlusPlusEstimator(Estimator):
+    """``KMeansPlusPlusEstimator(numMeans, maxIterations, stopTolerance, seed)`` (KMeansPlusPlus.scala:83-181): k-means++ seeding and
+    Lloyd passes on the device in fp64.  The seeding draws take ``numMeans`` uniforms from ``numpy.random.default_rng(seed)``, with the
+    draw rule of include/keystone_b200.h; Breeze's MersenneTwister stream is not reproduced.  After a fit ``seed_rows`` holds the
+    seed rows and ``stats`` the fit's statistics (cost history, stop reason, per-phase times)."""
+
+    def __init__(self, numMeans: int, maxIterations: int, stopTolerance: float = 1e-3, seed: int = 0, ctx: Optional[Context] = None):
+        self.num_means, self.max_iterations, self.stop_tolerance = int(numMeans), int(maxIterations), float(stopTolerance)
+        self.seed, self.ctx = seed, ctx
+        self.seed_rows: Optional[np.ndarray] = None
+        self.stats: Optional[dict] = None
+
+    def uniforms(self) -> np.ndarray:
+        return np.random.default_rng(self.seed).random(self.num_means)
+
+    def fit(self, data) -> KMeansModel:
+        x = _fit_rows(self.ctx, data)
+        u = self.uniforms()
+        means = np.zeros((self.num_means, x.cols))
+        seeds = np.zeros(self.num_means, dtype=np.int64)
+        it = C.c_int32(0)
+        check(x.ctx.handle, lib().ks_kmeans_fit(x.ctx.handle, x.handle, self.num_means, self.max_iterations, self.stop_tolerance,
+                                                 u.ctypes.data_as(C.c_void_p), means.ctypes.data_as(C.c_void_p),
+                                                 seeds.ctypes.data_as(C.c_void_p), C.byref(it)))
+        self.seed_rows, self.stats = seeds, x.ctx.last_fit_stats()
+        return KMeansModel(means, x.ctx)
+
+
+KMEANS_PLUS_PLUS_INITIALIZATION = "KMEANS_PLUS_PLUS_INITIALIZATION"
+RANDOM_INITIALIZATION = "RANDOM_INITIALIZATION"
+
+
+class GaussianMixtureModelEstimator(Estimator):
+    """``GaussianMixtureModelEstimator(k, maxIterations, minClusterSize, stopTolerance, weightThreshold, smallVarianceThreshold,
+    absoluteVarianceThreshold, initializationMethod, seed)`` (GaussianMixtureModelEstimator.scala): diagonal-covariance EM in fp64 on
+    the device, started from k-means++ (one Lloyd pass) or from random means.  The uniforms come from
+    ``numpy.random.default_rng(seed)`` (k of them for k-means++, k x dim for the random start); Breeze's stream is not reproduced.
+    The fitted ``GaussianMixtureModel`` carries the default weightThreshold 1e-4, as the reference's does, and already holds its
+    device copy for the fit's Context.  After a fit ``stats`` holds the iterations, stop reason and cost history."""
+
+    def __init__(self, k: int, maxIterations: int = 100, minClusterSize: int = 40, stopTolerance: float = 1e-4,
+                 weightThreshold: float = 1e-4, smallVarianceThreshold: float = 1e-2, absoluteVarianceThreshold: float = 1e-9,
+                 initializationMethod: str = KMEANS_PLUS_PLUS_INITIALIZATION, seed: int = 0, ctx: Optional[Context] = None):
+        if int(minClusterSize) <= 0:
+            raise ValueError("Minimum cluster size must be positive")
+        if int(maxIterations) <= 0:
+            raise ValueError("maxIterations must be positive")
+        if initializationMethod not in (KMEANS_PLUS_PLUS_INITIALIZATION, RANDOM_INITIALIZATION):
+            raise ValueError("initializationMethod must be KMEANS_PLUS_PLUS_INITIALIZATION or RANDOM_INITIALIZATION")
+        self.k, self.max_iterations, self.min_cluster_size = int(k), int(maxIterations), int(minClusterSize)
+        self.stop_tolerance, self.weight_threshold = float(stopTolerance), float(weightThreshold)
+        self.small_variance_threshold, self.absolute_variance_threshold = float(smallVarianceThreshold), float(absoluteVarianceThreshold)
+        self.initialization_method, self.seed, self.ctx = initializationMethod, seed, ctx
+        self.stats: Optional[dict] = None
+
+    def uniforms(self, dim: int) -> np.ndarray:
+        rng = np.random.default_rng(self.seed)
+        return rng.random(self.k) if self.initialization_method == KMEANS_PLUS_PLUS_INITIALIZATION else rng.random((self.k, int(dim)))
+
+    def fit(self, data) -> GaussianMixtureModel:
+        x = _fit_rows(self.ctx, data)
+        u = np.ascontiguousarray(self.uniforms(x.cols))
+        means, variances = np.zeros((x.cols, self.k), order="F"), np.zeros((x.cols, self.k), order="F")
+        weights = np.zeros(self.k)
+        h, it = C.c_int64(0), C.c_int32(0)
+        init = 0 if self.initialization_method == KMEANS_PLUS_PLUS_INITIALIZATION else 1
+        check(x.ctx.handle, lib().ks_gmm_fit(x.ctx.handle, x.handle, self.k, self.max_iterations, float(self.min_cluster_size),
+                                              self.stop_tolerance, self.weight_threshold, self.small_variance_threshold,
+                                              self.absolute_variance_threshold, init, u.ctypes.data_as(C.c_void_p), C.byref(h),
+                                              means.ctypes.data_as(C.c_void_p), variances.ctypes.data_as(C.c_void_p),
+                                              weights.ctypes.data_as(C.c_void_p), C.byref(it)))
+        owner = _GmmHandle(x.ctx, h.value)
+        self.stats = x.ctx.last_fit_stats()
+        gmm = GaussianMixtureModel(np.ascontiguousarray(means), np.ascontiguousarray(variances), weights)
+        gmm.ctx = x.ctx
+        gmm._handles[x.ctx.handle] = owner
+        return gmm
+
+
+class ScalaGMMFisherVectorEstimator(Estimator):
+    """``ScalaGMMFisherVectorEstimator(k)`` (FisherVector.scala:55-72): fits ``GaussianMixtureModelEstimator(k)`` with its defaults
+    on every descriptor of the items (an ``ItemBatch``'s rows, or the columns of (dim x n_i) matrices) and returns
+    ``FisherVector(gmm)``."""
+
+    def __init__(self, k: int, ctx: Optional[Context] = None):
+        self.k, self.ctx = int(k), ctx
+        self.gmm_estimator = GaussianMixtureModelEstimator(self.k, ctx=ctx)
+
+    def fit(self, data) -> FisherVector:
+        if not isinstance(data, ItemBatch):
+            if self.ctx is None:
+                raise KeystoneError(-1, "host items need a Context (pass ctx= to the estimator)")
+            data = ItemBatch.from_items(self.ctx, [data] if isinstance(data, np.ndarray) and data.ndim == 2 else list(data))
+        return FisherVector(self.gmm_estimator.fit(data))
+
+
+class GMMFisherVectorEstimator(ScalaGMMFisherVectorEstimator):
+    """``GMMFisherVectorEstimator(k)`` (FisherVector.scala:74-95).  The reference's optimizer switches to the EncEval C++ estimator
+    for k >= 32; that is a different algorithm and is not provided, so this always takes the Scala path (the device EM)."""
+
+
+class ColumnSampler(Transformer):
+    """``ColumnSampler(numSamplesPerMatrix)`` (K/nodes/stats/Sampling.scala:12-21): per item, ``numSamplesPerMatrix`` columns drawn
+    uniformly with replacement, gathered on the device into a new ``ItemBatch``.  Indices come from
+    ``numpy.random.default_rng(seed)`` (``seed=None``: fresh entropy, as the reference's unseeded ``scala.util.Random``)."""
+
+    def __init__(self, numSamplesPerMatrix: int, seed: Optional[int] = None, ctx: Optional[Context] = None):
+        if int(numSamplesPerMatrix) < 0:
+            raise ValueError("numSamplesPerMatrix must be >= 0")
+        self.num_samples, self.seed, self.ctx = int(numSamplesPerMatrix), seed, ctx
+        self._rng = np.random.default_rng(seed)
+
+    def sample_rows(self, offsets: np.ndarray) -> np.ndarray:
+        """The gathered rows of an item batch with these offsets (the next draws of this sampler's generator)."""
+        sizes = np.diff(np.asarray(offsets, dtype=np.int64))
+        if (sizes <= 0).any() and self.num_samples > 0:
+            raise ValueError("ColumnSampler: every item needs at least one column")
+        return np.concatenate([o + self._rng.integers(0, n, size=self.num_samples) for o, n in zip(offsets[:-1], sizes)]
+                              + [np.zeros(0, dtype=np.int64)]).astype(np.int64)
+
+    def apply(self, data):
+        if not isinstance(data, ItemBatch):
+            if self.ctx is None:
+                raise KeystoneError(-1, "host items need a Context (pass ctx= to the node)")
+            data = ItemBatch.from_items(self.ctx, list(data))
+        rows = np.ascontiguousarray(self.sample_rows(data.offsets))
+        h = C.c_int64(0)
+        check(data.ctx.handle, lib().ks_matrix_gather_rows(data.ctx.handle, data.matrix.handle, rows.ctypes.data_as(C.c_void_p), rows.size,
+                                                           C.byref(h)))
+        out = DeviceMatrix(data.ctx, h.value, rows.size, data.cols)
+        return ItemBatch(out, np.arange(data.n_items + 1, dtype=np.int64) * self.num_samples)

@@ -49,6 +49,15 @@ class KeystoneB200 extends Serializable {
   @native def gmmPosteriors(ctx: Long, gmm: Long, x: Long): Long
   @native def fisherVectorApply(ctx: Long, gmm: Long, descriptors: Long, itemOffsets: Array[Long]): Long
   @native def matrixNormalizeRows(ctx: Long, m: Long): Long
+  /** GMM EM, k-means++ and the row gather (not collective; DESIGN.md section 17).  uniforms: the header's draw rule; GMM means /
+   *  variances out: D x K DenseMatrix.data; k-means means out: numMeans x dim row-major. */
+  @native def gmmFit(ctx: Long, x: Long, k: Long, maxIterations: Int, minClusterSize: Double, stopTolerance: Double,
+      weightThreshold: Double, smallVarianceThreshold: Double, absoluteVarianceThreshold: Double, initialization: Int,
+      uniforms: Array[Double], meansOut: Array[Double], variancesOut: Array[Double], weightsOut: Array[Double]): Long
+  @native def kmeansFit(ctx: Long, x: Long, numMeans: Long, maxIterations: Int, stopTolerance: Double, uniforms: Array[Double],
+      meansOut: Array[Double]): Int
+  @native def kmeansAssign(ctx: Long, x: Long, meansRowMajor: Array[Double], numMeans: Long, dim: Long): Long
+  @native def matrixGatherRows(ctx: Long, m: Long, rows: Array[Long]): Long
   @native def matrixSignedSqrt(ctx: Long, m: Long): Long
 
   @native def modelFromHost(ctx: Long, xs: Array[Array[Double]], blockSize: Int, k: Long, b: Array[Double],
