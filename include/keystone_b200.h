@@ -200,6 +200,31 @@ KS_API int32_t ks_gmm_fit(int64_t ctx, int64_t x, int64_t k, int32_t max_iterati
 /* out = rows rows[0..n) of m, in that order, as a new matrix (ColumnSampler on an item batch); indices must lie in [0, rows). */
 KS_API int32_t ks_matrix_gather_rows(int64_t ctx, int64_t m, const int64_t* rows, int64_t n, int64_t* out_m);
 
+/* ---- PixelScaler, GrayScaler and dense multi-scale SIFT (DESIGN.md section 18) -----------------------------------------------
+ * The first three nodes of K/pipelines/images/voc/VOCSIFTFisher.scala and of the SIFT half of ImageNetSiftLcsFV.scala.  Images are
+ * rows in ImageVectorizer order (value (x, y, c) at c + x*channels + y*channels*x_dim, x_dim = image height), all of one shape.
+ * Non-finite pixels are rejected with KS_ERR_INVALID.  None of these is collective. */
+/* PixelScaler (K/nodes/images/PixelScaler.scala): every value / 255.0 in fp64, rounded once to fp32; a new matrix. */
+KS_API int32_t ks_image_pixel_scale(int64_t ctx, int64_t images, int64_t* out_m);
+/* GrayScaler (ImageUtils.toGrayScale), after PixelScaler when pixel_scale is 1: in fp64, 0.2989 R + 0.5870 G + 0.1140 B with B at
+ * channel 0 for three channels, sqrt(sum_c v^2 / channels) otherwise; rounded once to fp32.  Output: one-channel images,
+ * n_images x (x_dim * y_dim).  Rejects bad shapes and pixel_scale outside {0, 1}. */
+KS_API int32_t ks_image_grayscale(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, int32_t pixel_scale,
+                                  int64_t* out_m);
+/* SIFTExtractor(step, bin, scales, scale_step).apply (K/nodes/images/external/SIFTExtractor.scala) on one-channel images
+ * (n_images x (x_dim * y_dim)): vlfeat's dense SIFT with a flat window at every scale s < scales (bin + 2s, step + s*scale_step),
+ * the contrast threshold 0.005 and the reference's transposed uint8 quantisation.  Output: (n_images * nKP) x 128 fp32 holding
+ * integers in [0, 255], one descriptor per ROW (the reference's columns); image i owns rows [i nKP, (i+1) nKP), scales follow in
+ * order, and within a scale frames run along y outer, x inner, as vlfeat (which sees the image transposed) emits them.  A scale
+ * without frames contributes no rows.  Rejects bad shapes, step < 1, bin < 1, scales < 1, scale_step < 0 and oversized
+ * parameters (step, scale_step > 65536, bin > 4096, scales > 256). */
+KS_API int32_t ks_sift_extract(int64_t ctx, int64_t gray_images, int32_t x_dim, int32_t y_dim, int32_t step, int32_t bin, int32_t scales,
+                               int32_t scale_step, int64_t* out_m);
+/* Host only: counts_out[s] (scales entries) = the keypoints ks_sift_extract emits per image at scale s.  Returns KS_ERR_INVALID
+ * for the arguments ks_sift_extract rejects. */
+KS_API int32_t ks_sift_keypoints(int32_t x_dim, int32_t y_dim, int32_t step, int32_t bin, int32_t scales, int32_t scale_step,
+                                 int64_t* counts_out);
+
 /* ---- Convolver [andThen SymmetricRectifier andThen Pooler(sum) andThen ImageVectorizer] ---------------------------------
  * The featurizer of K/pipelines/images/cifar/RandomPatchCifar.scala:59-63 (K/nodes/images/Convolver.scala:20-203,
  * SymmetricRectifier.scala:7-32, Pooler.scala:21-69, K/utils/Stats.scala:112-123).  filters: DenseMatrix (n_filters x

@@ -14,6 +14,8 @@
 //       -Lkeystone_b200/lib -lkeystone_b200 -o lib/libkeystone_b200_jni.so
 #include <jni.h>
 
+#include <vector>
+
 #include "keystone_b200.h"
 
 #define JFN(ret, name) extern "C" JNIEXPORT ret JNICALL Java_keystoneml_nodes_learning_gpu_KeystoneB200_##name
@@ -260,6 +262,29 @@ JFN(jlong, matrixGatherRows)(JNIEnv* env, jobject, jlong ctx, jlong m, jlongArra
   int64_t h = 0;
   LongArray r(env, rows);
   return ok(env, ctx, ks_matrix_gather_rows(ctx, m, r.data(), r.n, &h)) ? h : 0;
+}
+// ---- PixelScaler, GrayScaler, dense SIFT (not collective)
+JFN(jlong, imagePixelScale)(JNIEnv* env, jobject, jlong ctx, jlong images) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_image_pixel_scale(ctx, images, &h)) ? h : 0;
+}
+JFN(jlong, imageGrayscale)(JNIEnv* env, jobject, jlong ctx, jlong images, jint xDim, jint yDim, jint channels, jint pixelScale) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_image_grayscale(ctx, images, xDim, yDim, channels, pixelScale, &h)) ? h : 0;
+}
+JFN(jlong, siftExtract)(JNIEnv* env, jobject, jlong ctx, jlong grayImages, jint xDim, jint yDim, jint step, jint bin, jint scales,
+                        jint scaleStep) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_sift_extract(ctx, grayImages, xDim, yDim, step, bin, scales, scaleStep, &h)) ? h : 0;
+}
+// per-scale keypoint counts (host only); null when the arguments are rejected
+JFN(jlongArray, siftKeypoints)(JNIEnv* env, jobject, jint xDim, jint yDim, jint step, jint bin, jint scales, jint scaleStep) {
+  if (scales < 1) return nullptr;
+  std::vector<int64_t> counts(static_cast<size_t>(scales));
+  if (ks_sift_keypoints(xDim, yDim, step, bin, scales, scaleStep, counts.data()) != KS_OK) return nullptr;
+  jlongArray out = env->NewLongArray(scales);
+  if (out) env->SetLongArrayRegion(out, 0, scales, reinterpret_cast<const jlong*>(counts.data()));
+  return out;
 }
 JFN(jlong, matrixNormalizeRows)(JNIEnv* env, jobject, jlong ctx, jlong m) {
   int64_t h = 0;

@@ -97,6 +97,10 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_kmeans_assign", i64, i64, C.c_void_p, i64, i64, p_i64)
     sig("ks_gmm_fit", i64, i64, i64, i32, f64, f64, f64, f64, f64, i32, C.c_void_p, p_i64, C.c_void_p, C.c_void_p, C.c_void_p, p_i32)
     sig("ks_matrix_gather_rows", i64, i64, C.c_void_p, i64, p_i64)
+    sig("ks_image_pixel_scale", i64, i64, p_i64)
+    sig("ks_image_grayscale", i64, i64, i32, i32, i32, i32, p_i64)
+    sig("ks_sift_extract", i64, i64, i32, i32, i32, i32, i32, i32, p_i64)
+    sig("ks_sift_keypoints", i32, i32, i32, i32, i32, i32, p_i64)
     sig("ks_blockls_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, i64, i32, p_i64)
     sig("ks_blockwls_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, f64, i64, i32, p_i64)
     sig("ks_linear_map_fit", i64, i64, i64, i32, f64, p_i64)

@@ -2167,6 +2167,39 @@ KS_API int32_t ks_matrix_gather_rows(int64_t ctx, int64_t m, const int64_t* rows
   });
 }
 
+// ---------------------------------------------------------------- PixelScaler, GrayScaler, SIFT (sift.cu)
+KS_API int32_t ks_image_pixel_scale(int64_t ctx, int64_t images, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(image_pixel_scale(c, c.matrix(images)));
+  });
+}
+KS_API int32_t ks_image_grayscale(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, int32_t pixel_scale,
+                                  int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(image_grayscale(c, c.matrix(images), x_dim, y_dim, channels, pixel_scale));
+  });
+}
+KS_API int32_t ks_sift_extract(int64_t ctx, int64_t gray_images, int32_t x_dim, int32_t y_dim, int32_t step, int32_t bin, int32_t scales,
+                               int32_t scale_step, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(sift_extract(c, c.matrix(gray_images), x_dim, y_dim, step, bin, scales, scale_step));
+  });
+}
+KS_API int32_t ks_sift_keypoints(int32_t x_dim, int32_t y_dim, int32_t step, int32_t bin, int32_t scales, int32_t scale_step,
+                                 int64_t* counts_out) {
+  if (!counts_out) return KS_ERR_INVALID;
+  try {
+    const std::vector<SiftScale> g = sift_geometry(x_dim, y_dim, step, bin, scales, scale_step);
+    for (size_t s = 0; s < g.size(); ++s) counts_out[s] = static_cast<int64_t>(g[s].nfx) * g[s].nfy;
+  } catch (const KsError& e) {
+    return e.code;
+  }
+  return KS_OK;
+}
+
 // ---------------------------------------------------------------- models
 KS_API int32_t ks_model_from_host(int64_t ctx, const double* const* xs, const int64_t* block_rows, int32_t n_blocks, int64_t k,
                            const double* b_or_null, const double* const* means_or_null, int32_t block_size, int64_t* out_model) {

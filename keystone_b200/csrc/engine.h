@@ -419,4 +419,15 @@ struct GmmFitArgs {
 int64_t gmm_fit(Ctx& c, Matrix& X, const GmmFitArgs& a, double* means_colmajor, double* vars_colmajor, double* weights, int* iterations);
 std::unique_ptr<Matrix> gather_rows(Ctx& c, Matrix& X, const int64_t* rows, int64_t n);
 
+// PixelScaler, GrayScaler and dense multi-scale SIFT (sift.cu); none is collective
+struct SiftScale {
+  int b = 0, st = 0, lo = 0;  // bin size, step and first frame coordinate of the scale
+  int nfx = 0, nfy = 0;       // frames along x (vlfeat's x, the Image's rows) and y
+};
+// validates the parameters (throws KS_ERR_INVALID) and returns the per-scale geometry; host only
+std::vector<SiftScale> sift_geometry(int x_dim, int y_dim, int step, int bin, int scales, int scale_step);
+std::unique_ptr<Matrix> image_pixel_scale(Ctx& c, Matrix& images);
+std::unique_ptr<Matrix> image_grayscale(Ctx& c, Matrix& images, int x_dim, int y_dim, int channels, int pixel_scale);
+std::unique_ptr<Matrix> sift_extract(Ctx& c, Matrix& gray_images, int x_dim, int y_dim, int step, int bin, int scales, int scale_step);
+
 }  // namespace ks

@@ -1537,3 +1537,155 @@ class ColumnSampler(Transformer):
                                                            C.byref(h)))
         out = DeviceMatrix(data.ctx, h.value, rows.size, data.cols)
         return ItemBatch(out, np.arange(data.n_items + 1, dtype=np.int64) * self.num_samples)
+
+
+# ------------------------------------------------------------------------------------------------- dense SIFT branch
+# PixelScaler -> GrayScaler -> SIFTExtractor, the head of K/pipelines/images/voc/VOCSIFTFisher.scala:41-44 and of the SIFT half of
+# K/pipelines/images/imagenet/ImageNetSiftLcsFV.scala:99-101.  DESIGN.md section 18.
+def _new_matrix(ctx: Context, handle: int) -> DeviceMatrix:
+    rows, cols = C.c_int64(0), C.c_int64(0)
+    check(ctx.handle, lib().ks_matrix_shape(ctx.handle, handle, C.byref(rows), C.byref(cols)))
+    return DeviceMatrix(ctx, handle, rows.value, cols.value)
+
+
+class _PixelScaledImages(ImageBatch):
+    """PixelScaler's output: the source batch with x / 255.0 pending, so that GrayScaler can take it in fp64 together with the gray
+    weights (the reference never rounds in between).  Reading ``matrix`` materialises the scaled values, rounded once to fp32."""
+
+    def __init__(self, source: ImageBatch):
+        self.ctx, self.source = source.ctx, source
+        self.x_dim, self.y_dim, self.channels = source.x_dim, source.y_dim, source.channels
+        self._matrix: Optional[DeviceMatrix] = None
+
+    @property
+    def matrix(self) -> DeviceMatrix:
+        if self._matrix is None:
+            h = C.c_int64(0)
+            check(self.ctx.handle, lib().ks_image_pixel_scale(self.ctx.handle, self.source.matrix.handle, C.byref(h)))
+            self._matrix = _new_matrix(self.ctx, h.value)
+        return self._matrix
+
+    @property
+    def rows(self) -> int:
+        return self.source.rows
+
+
+def _image_batches(node, data):
+    """Image inputs as (batches, restore): an ImageBatch, an (n, x, y, c) array, one (x, y, c) or (x, y) image, or a list of images and
+    batches (one batch per shape); restore(per-batch results) puts per-image results back in input order."""
+    def upload(a):
+        if node.ctx is None:
+            raise KeystoneError(-1, "numpy input needs a Context (pass ctx= to the node)")
+        return ImageBatch.from_images(node.ctx, a)
+
+    if isinstance(data, ImageBatch):
+        return [data], None
+    if isinstance(data, np.ndarray) and data.ndim == 4:
+        return [upload(data)], None
+    if isinstance(data, np.ndarray) and data.ndim in (2, 3):
+        a = data if data.ndim == 3 else data[:, :, None]
+        return [upload(a[None])], "single"
+    items = list(data)
+    groups = {}
+    for i, im in enumerate(items):
+        key = ("batch", i) if isinstance(im, ImageBatch) else np.asarray(im).shape
+        groups.setdefault(key, []).append(i)
+    batches, order = [], []
+    for key, idx in groups.items():
+        if key[0] == "batch":
+            batches.append(items[idx[0]])
+        else:
+            ims = [np.asarray(items[i]) for i in idx]
+            batches.append(upload(np.stack([m if m.ndim == 3 else m[:, :, None] for m in ims])))
+        order.append(idx)
+    return batches, order
+
+
+def _per_batch(node, data, fn):
+    """fn on an ImageBatch, on an array uploaded as one, or on each image of a list (a list of one-image batches, input order)."""
+    if isinstance(data, (list, tuple)):
+        return [fn(b if isinstance(b, ImageBatch) else _image_batches(node, np.asarray(b))[0][0]) for b in data]
+    return fn(_image_batches(node, data)[0][0])
+
+
+class PixelScaler(Transformer):
+    """``PixelScaler`` (K/nodes/images/PixelScaler.scala): every value / 255.0, in fp64.  ImageBatch -> ImageBatch; the division is
+    deferred so that a following GrayScaler computes both in fp64 and rounds once."""
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx
+
+    def apply(self, data):
+        return _per_batch(self, data, _PixelScaledImages)
+
+
+class GrayScaler(Transformer):
+    """``GrayScaler`` (K/nodes/images/GrayScaler.scala, ImageUtils.toGrayScale): 0.2989 R + 0.5870 G + 0.1140 B with the channels in
+    BGR order for three channels, sqrt(mean of squares) otherwise, in fp64 (after PixelScaler's division when one precedes it),
+    rounded once to fp32.  ImageBatch -> one-channel ImageBatch."""
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx
+
+    @staticmethod
+    def _gray(batch: ImageBatch) -> ImageBatch:
+        scaled = isinstance(batch, _PixelScaledImages) and batch._matrix is None
+        src = batch.source if scaled else batch
+        h = C.c_int64(0)
+        check(batch.ctx.handle, lib().ks_image_grayscale(batch.ctx.handle, src.matrix.handle, batch.x_dim, batch.y_dim, batch.channels,
+                                                         1 if scaled else 0, C.byref(h)))
+        return ImageBatch(_new_matrix(batch.ctx, h.value), batch.x_dim, batch.y_dim, 1)
+
+    def apply(self, data):
+        return _per_batch(self, data, self._gray)
+
+
+class SIFTExtractor(Transformer):
+    """``SIFTExtractor(stepSize, binSize, scales, scaleStep)`` (K/nodes/images/external/SIFTExtractor.scala): vlfeat's dense SIFT with a
+    flat window at ``scales`` scales (bin ``binSize + 2s``, step ``stepSize + s scaleStep``), 128 integer values in [0, 255] per
+    keypoint, zero below the contrast threshold.  Input: one-channel images -- an ``ImageBatch``, an (n, x, y, 1) array, one (x, y[, 1])
+    image (returns its (128 x nKP) matrix, as the reference) or a list of images, grouped by shape, input order kept.  Output: an
+    ``ItemBatch`` with one item per image, one descriptor per row."""
+
+    descriptorSize = 128
+
+    def __init__(self, stepSize: int = 3, binSize: int = 4, scales: int = 4, scaleStep: int = 1, ctx: Optional[Context] = None):
+        self.step, self.bin, self.scales, self.scale_step, self.ctx = int(stepSize), int(binSize), int(scales), int(scaleStep), ctx
+
+    def keypoints_per_scale(self, x_dim: int, y_dim: int) -> List[int]:
+        counts = np.zeros(max(self.scales, 1), dtype=np.int64)
+        rc = lib().ks_sift_keypoints(x_dim, y_dim, self.step, self.bin, self.scales, self.scale_step, counts.ctypes.data_as(_capi.p_i64))
+        if rc != 0:
+            raise KeystoneError(rc, "SIFTExtractor: invalid image shape or parameters (stepSize, binSize, scales >= 1, scaleStep >= 0)")
+        return [int(v) for v in counts[:self.scales]]
+
+    def keypoints(self, x_dim: int, y_dim: int) -> int:
+        return sum(self.keypoints_per_scale(x_dim, y_dim))
+
+    def _extract(self, batch: ImageBatch) -> ItemBatch:
+        if batch.channels != 1:
+            raise KeystoneError(-1, "SIFTExtractor: the images must have one channel (apply GrayScaler first)")
+        nkp = self.keypoints(batch.x_dim, batch.y_dim)
+        h = C.c_int64(0)
+        check(batch.ctx.handle, lib().ks_sift_extract(batch.ctx.handle, batch.matrix.handle, batch.x_dim, batch.y_dim, self.step, self.bin,
+                                                      self.scales, self.scale_step, C.byref(h)))
+        return ItemBatch(_new_matrix(batch.ctx, h.value), np.arange(batch.rows + 1, dtype=np.int64) * nkp)
+
+    def apply(self, data):
+        batches, order = _image_batches(self, data)
+        if order is None:
+            return self._extract(batches[0])
+        if order == "single":
+            return self._extract(batches[0]).to_list(np.float32)[0]
+        if len(batches) == 1 and isinstance(data, (list, tuple)) and not isinstance(data[0], ImageBatch):
+            return self._extract(batches[0])
+        # several batches: one extraction each, the items put back in input order on the host
+        n = sum(len(idx) for idx in order)
+        items: List[Optional[np.ndarray]] = [None] * n
+        for b, idx in zip(batches, order):
+            got = self._extract(b).to_list(np.float32)
+            if len(got) != len(idx):
+                raise ValueError("SIFTExtractor: an ImageBatch inside a list must hold exactly one image")
+            for i, m in zip(idx, got):
+                items[i] = m
+        return ItemBatch.from_items(batches[0].ctx, items)

@@ -59,6 +59,12 @@ class KeystoneB200 extends Serializable {
   @native def kmeansAssign(ctx: Long, x: Long, meansRowMajor: Array[Double], numMeans: Long, dim: Long): Long
   @native def matrixGatherRows(ctx: Long, m: Long, rows: Array[Long]): Long
   @native def matrixSignedSqrt(ctx: Long, m: Long): Long
+  /** PixelScaler, GrayScaler and dense SIFT (not collective; DESIGN.md section 18).  siftKeypoints is host only: the per-scale
+   *  keypoint counts, or null for rejected arguments. */
+  @native def imagePixelScale(ctx: Long, images: Long): Long
+  @native def imageGrayscale(ctx: Long, images: Long, xDim: Int, yDim: Int, channels: Int, pixelScale: Int): Long
+  @native def siftExtract(ctx: Long, grayImages: Long, xDim: Int, yDim: Int, step: Int, bin: Int, scales: Int, scaleStep: Int): Long
+  @native def siftKeypoints(xDim: Int, yDim: Int, step: Int, bin: Int, scales: Int, scaleStep: Int): Array[Long]
 
   @native def modelFromHost(ctx: Long, xs: Array[Array[Double]], blockSize: Int, k: Long, b: Array[Double],
       means: Array[Array[Double]]): Long
