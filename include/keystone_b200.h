@@ -225,6 +225,26 @@ KS_API int32_t ks_sift_extract(int64_t ctx, int64_t gray_images, int32_t x_dim, 
 KS_API int32_t ks_sift_keypoints(int32_t x_dim, int32_t y_dim, int32_t step, int32_t bin, int32_t scales, int32_t scale_step,
                                  int64_t* counts_out);
 
+/* ---- HOG and DAISY descriptors (DESIGN.md section 19) --------------------------------------------------------------------------
+ * Images as for SIFT above: rows in ImageVectorizer order, all of one shape; image i owns a contiguous row range of the output, and
+ * an image with no cell or keypoint contributes no rows.  Non-finite pixels are rejected with KS_ERR_INVALID.  Not collective. */
+/* HogExtractor(bin).apply (K/nodes/images/HogExtractor.scala) on three-channel BGR images, after PixelScaler when pixel_scale is 1
+ * (x / 255.0 in fp64, never rounded).  nX = round(x_dim / bin), nY = round(y_dim / bin) cells; output (n_images * (nX-2)(nY-2)) x 32
+ * fp32, the reference's cells x 32 matrix per image with row y + x (nY - 2): 18 contrast-sensitive, 9 contrast-insensitive and 4
+ * texture values and a zero.  Reads past the visible edge are the reference's unclamped reads of c + x*3 + y*3*x_dim; rejects bin
+ * and shape pairs where such a read passes the end of the image, channels != 3, bin outside [1, 1024], bad shapes and pixel_scale
+ * outside {0, 1}. */
+KS_API int32_t ks_hog_extract(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, int32_t pixel_scale, int32_t bin,
+                              int64_t* out_m);
+/* DaisyExtractor(T, Q, R, H, border, stride).apply (K/nodes/images/DaisyExtractor.scala) on one-channel images: gradients, H
+ * rectified orientation maps and Q Gaussian blur layers in fp64 (ImageUtils.conv2D), keypoints x = border .. x_dim-border-1 by
+ * stride outer, y likewise inner.  Output: (n_images * nKP) x (H (T Q + 1)) fp32, one keypoint per ROW (the reference's columns):
+ * the centre histogram at columns [0, H), ring sample (l, t) at H + t Q H + l H, each normalised to unit L2 norm or zeroed when its
+ * norm is <= 1e-8.  Rejects T, Q, R, H, stride < 1, border < 0, oversized parameters (T, H > 64, Q > 16, R > 4096, a blur radius
+ * > 1024, stride or border > 65536), ring samples that leave the image and bad shapes. */
+KS_API int32_t ks_daisy_extract(int64_t ctx, int64_t gray_images, int32_t x_dim, int32_t y_dim, int32_t T, int32_t Q, int32_t R, int32_t H,
+                                int32_t border, int32_t stride, int64_t* out_m);
+
 /* ---- Convolver [andThen SymmetricRectifier andThen Pooler(sum) andThen ImageVectorizer] ---------------------------------
  * The featurizer of K/pipelines/images/cifar/RandomPatchCifar.scala:59-63 (K/nodes/images/Convolver.scala:20-203,
  * SymmetricRectifier.scala:7-32, Pooler.scala:21-69, K/utils/Stats.scala:112-123).  filters: DenseMatrix (n_filters x

@@ -286,6 +286,16 @@ JFN(jlongArray, siftKeypoints)(JNIEnv* env, jobject, jint xDim, jint yDim, jint 
   if (out) env->SetLongArrayRegion(out, 0, scales, reinterpret_cast<const jlong*>(counts.data()));
   return out;
 }
+// ---- HOG and DAISY (not collective)
+JFN(jlong, hogExtract)(JNIEnv* env, jobject, jlong ctx, jlong images, jint xDim, jint yDim, jint channels, jint pixelScale, jint bin) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_hog_extract(ctx, images, xDim, yDim, channels, pixelScale, bin, &h)) ? h : 0;
+}
+JFN(jlong, daisyExtract)(JNIEnv* env, jobject, jlong ctx, jlong grayImages, jint xDim, jint yDim, jint daisyT, jint daisyQ, jint daisyR,
+                         jint daisyH, jint pixelBorder, jint stride) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_daisy_extract(ctx, grayImages, xDim, yDim, daisyT, daisyQ, daisyR, daisyH, pixelBorder, stride, &h)) ? h : 0;
+}
 JFN(jlong, matrixNormalizeRows)(JNIEnv* env, jobject, jlong ctx, jlong m) {
   int64_t h = 0;
   return ok(env, ctx, ks_matrix_normalize_rows(ctx, m, &h)) ? h : 0;

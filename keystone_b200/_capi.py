@@ -101,6 +101,8 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_image_grayscale", i64, i64, i32, i32, i32, i32, p_i64)
     sig("ks_sift_extract", i64, i64, i32, i32, i32, i32, i32, i32, p_i64)
     sig("ks_sift_keypoints", i32, i32, i32, i32, i32, i32, p_i64)
+    sig("ks_hog_extract", i64, i64, i32, i32, i32, i32, i32, p_i64)
+    sig("ks_daisy_extract", i64, i64, i32, i32, i32, i32, i32, i32, i32, i32, p_i64)
     sig("ks_blockls_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, i64, i32, p_i64)
     sig("ks_blockwls_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, f64, i64, i32, p_i64)
     sig("ks_linear_map_fit", i64, i64, i64, i32, f64, p_i64)

@@ -2200,6 +2200,22 @@ KS_API int32_t ks_sift_keypoints(int32_t x_dim, int32_t y_dim, int32_t step, int
   return KS_OK;
 }
 
+// ---------------------------------------------------------------- HOG, DAISY (hog_daisy.cu)
+KS_API int32_t ks_hog_extract(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, int32_t pixel_scale, int32_t bin,
+                              int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(hog_extract(c, c.matrix(images), x_dim, y_dim, channels, pixel_scale, bin));
+  });
+}
+KS_API int32_t ks_daisy_extract(int64_t ctx, int64_t gray_images, int32_t x_dim, int32_t y_dim, int32_t T, int32_t Q, int32_t R, int32_t H,
+                                int32_t border, int32_t stride, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(daisy_extract(c, c.matrix(gray_images), x_dim, y_dim, T, Q, R, H, border, stride));
+  });
+}
+
 // ---------------------------------------------------------------- models
 KS_API int32_t ks_model_from_host(int64_t ctx, const double* const* xs, const int64_t* block_rows, int32_t n_blocks, int64_t k,
                            const double* b_or_null, const double* const* means_or_null, int32_t block_size, int64_t* out_model) {

@@ -429,5 +429,24 @@ std::vector<SiftScale> sift_geometry(int x_dim, int y_dim, int step, int bin, in
 std::unique_ptr<Matrix> image_pixel_scale(Ctx& c, Matrix& images);
 std::unique_ptr<Matrix> image_grayscale(Ctx& c, Matrix& images, int x_dim, int y_dim, int channels, int pixel_scale);
 std::unique_ptr<Matrix> sift_extract(Ctx& c, Matrix& gray_images, int x_dim, int y_dim, int step, int bin, int scales, int scale_step);
+// throws KS_ERR_INVALID naming `who` when any of the first `cols` values of a row of m is not finite (sift.cu)
+void check_finite(Ctx& c, const Matrix& m, int64_t cols, const char* who);
+
+// HOG and DAISY descriptors (hog_daisy.cu); neither is collective
+struct HogShape {
+  int nx = 0, ny = 0;  // cells along x (the Image's rows) and y: Scala's round(dim / bin)
+  int64_t rows = 0;    // feature rows per image, (nx - 2)(ny - 2) or 0
+};
+// validates the shape and bin (throws KS_ERR_INVALID), including the reference's out-of-image read; host only
+HogShape hog_shape(int x_dim, int y_dim, int channels, int bin);
+std::unique_ptr<Matrix> hog_extract(Ctx& c, Matrix& images, int x_dim, int y_dim, int channels, int pixel_scale, int bin);
+struct DaisyShape {
+  int nkx = 0, nky = 0, features = 0;     // keypoints along x and y; H (T Q + 1)
+  std::vector<std::vector<double>> taps;  // the Gaussian taps of each blur layer
+  std::vector<int> samples;               // (dx, dy, layer) of each histogram, the centre first, then ring sample (t, l) at 1 + t Q + l
+};
+// validates the parameters (throws KS_ERR_INVALID), including ring samples that leave the image; host only
+DaisyShape daisy_shape(int x_dim, int y_dim, int T, int Q, int R, int H, int border, int stride);
+std::unique_ptr<Matrix> daisy_extract(Ctx& c, Matrix& gray_images, int x_dim, int y_dim, int T, int Q, int R, int H, int border, int stride);
 
 }  // namespace ks

@@ -278,7 +278,7 @@ static float bin_window_mean(int bin, int index) {  // _vl_dsift_get_bin_window_
   return acc / static_cast<float>(2 * bin - 1);
 }
 
-static void check_finite(Ctx& c, const Matrix& m, int64_t cols, const char* who) {
+void check_finite(Ctx& c, const Matrix& m, int64_t cols, const char* who) {
   if (m.rows == 0) return;
   DevBuf flag;
   flag.alloc(sizeof(unsigned));

@@ -1689,3 +1689,90 @@ class SIFTExtractor(Transformer):
             for i, m in zip(idx, got):
                 items[i] = m
         return ItemBatch.from_items(batches[0].ctx, items)
+
+
+# ---------------------------------------------------------------------------------------------------------------- HOG and DAISY
+# K/nodes/images/{HogExtractor,DaisyExtractor}.scala.  DESIGN.md section 19.
+def _items_in_input_order(node, data, extract, single):
+    """extract(ImageBatch) -> ItemBatch over the inputs _image_batches accepts; one image gives single(that ItemBatch), and a list
+    that needed several batches is put back in input order on the host."""
+    batches, order = _image_batches(node, data)
+    if order is None:
+        return extract(batches[0])
+    if order == "single":
+        return single(extract(batches[0]))
+    if len(batches) == 1 and isinstance(data, (list, tuple)) and not isinstance(data[0], ImageBatch):
+        return extract(batches[0])
+    rows: List[Optional[np.ndarray]] = [None] * sum(len(idx) for idx in order)
+    for b, idx in zip(batches, order):
+        got = extract(b)
+        if got.n_items != len(idx):
+            raise ValueError(f"{type(node).__name__}: an ImageBatch inside a list must hold exactly one image")
+        host = got.to_numpy(np.float32)
+        for k, i in enumerate(idx):
+            rows[i] = host[got.offsets[k]:got.offsets[k + 1]]
+    return ItemBatch(batches[0].ctx.matrix(np.concatenate(rows, 0)), np.cumsum([0] + [r.shape[0] for r in rows]))
+
+
+def _item_batch(batch: ImageBatch, handle: int) -> ItemBatch:
+    m = _new_matrix(batch.ctx, handle)
+    per = m.rows // batch.rows if batch.rows else 0
+    return ItemBatch(m, np.arange(batch.rows + 1, dtype=np.int64) * per)
+
+
+class HogExtractor(Transformer):
+    """``new HogExtractor(binSize)`` (K/nodes/images/HogExtractor.scala, voc-release5's features.cc): per interior cell of
+    round(xDim / bin) x round(yDim / bin) cells, 18 contrast-sensitive, 9 contrast-insensitive and 4 texture values and a zero.
+    Input: three-channel BGR images, usually PixelScaler's output (its x / 255.0 is then taken in fp64 with the gradients, as the
+    reference never rounds it) -- an ``ImageBatch``, an (n, x, y, 3) array, one (x, y, 3) image (returns the reference's (cells x 32)
+    matrix) or a list of images, grouped by shape, input order kept.  Output: an ``ItemBatch`` with one item per image and one cell
+    per row, row y + x (nY - 2)."""
+
+    numFeatures = 32
+
+    def __init__(self, binSize: int, ctx: Optional[Context] = None):
+        self.bin, self.ctx = int(binSize), ctx
+
+    def cells(self, x_dim: int, y_dim: int) -> int:
+        """Feature rows per image: (nX - 2)(nY - 2), with nX = round(x_dim / bin) as Scala rounds (floor(v + 0.5))."""
+        nx, ny = (int(np.floor(d / self.bin + 0.5)) for d in (x_dim, y_dim))
+        return max(nx - 2, 0) * max(ny - 2, 0)
+
+    def _extract(self, batch: ImageBatch) -> ItemBatch:
+        scaled = isinstance(batch, _PixelScaledImages) and batch._matrix is None
+        src = batch.source if scaled else batch
+        h = C.c_int64(0)
+        check(batch.ctx.handle, lib().ks_hog_extract(batch.ctx.handle, src.matrix.handle, batch.x_dim, batch.y_dim, batch.channels,
+                                                     1 if scaled else 0, self.bin, C.byref(h)))
+        return _item_batch(batch, h.value)
+
+    def apply(self, data):
+        return _items_in_input_order(self, data, self._extract, lambda items: items.to_numpy(np.float32))
+
+
+class DaisyExtractor(Transformer):
+    """``new DaisyExtractor(daisyT, daisyQ, daisyR, daisyH, pixelBorder, stride, patchSize)`` (K/nodes/images/DaisyExtractor.scala):
+    per keypoint (x = pixelBorder .. xDim - pixelBorder - 1 by stride outer, y likewise inner) the centre histogram and daisyT x daisyQ
+    ring histograms of daisyH rectified, Gaussian-blurred orientation maps, each L2-normalised in fp64 (``daisyFeatureSize`` =
+    daisyH (daisyT daisyQ + 1) values).  ``patchSize`` is unused, as in the reference.  Input: one-channel images (GrayScaler's
+    output), accepted as by ``SIFTExtractor``; one image returns its (daisyFeatureSize x nKP) matrix, as the reference.  Output: an
+    ``ItemBatch`` with one item per image, one keypoint per row."""
+
+    def __init__(self, daisyT: int = 8, daisyQ: int = 3, daisyR: int = 7, daisyH: int = 8, pixelBorder: int = 16, stride: int = 4,
+                 patchSize: int = 24, ctx: Optional[Context] = None):
+        self.daisyT, self.daisyQ, self.daisyR, self.daisyH = int(daisyT), int(daisyQ), int(daisyR), int(daisyH)
+        self.pixelBorder, self.stride, self.patchSize, self.ctx = int(pixelBorder), int(stride), int(patchSize), ctx
+        self.daisyFeatureSize = self.daisyH * (self.daisyT * self.daisyQ + 1)
+
+    def keypoints(self, x_dim: int, y_dim: int) -> int:
+        return len(range(self.pixelBorder, x_dim - self.pixelBorder, self.stride)) * \
+            len(range(self.pixelBorder, y_dim - self.pixelBorder, self.stride))
+
+    def _extract(self, batch: ImageBatch) -> ItemBatch:
+        h = C.c_int64(0)
+        check(batch.ctx.handle, lib().ks_daisy_extract(batch.ctx.handle, batch.matrix.handle, batch.x_dim, batch.y_dim, self.daisyT,
+                                                       self.daisyQ, self.daisyR, self.daisyH, self.pixelBorder, self.stride, C.byref(h)))
+        return _item_batch(batch, h.value)
+
+    def apply(self, data):
+        return _items_in_input_order(self, data, self._extract, lambda items: items.to_list(np.float32)[0])

@@ -65,6 +65,10 @@ class KeystoneB200 extends Serializable {
   @native def imageGrayscale(ctx: Long, images: Long, xDim: Int, yDim: Int, channels: Int, pixelScale: Int): Long
   @native def siftExtract(ctx: Long, grayImages: Long, xDim: Int, yDim: Int, step: Int, bin: Int, scales: Int, scaleStep: Int): Long
   @native def siftKeypoints(xDim: Int, yDim: Int, step: Int, bin: Int, scales: Int, scaleStep: Int): Array[Long]
+  /** HOG (pixelScale = 1 takes PixelScaler's x / 255.0 in fp64) and DAISY (not collective; DESIGN.md section 19). */
+  @native def hogExtract(ctx: Long, images: Long, xDim: Int, yDim: Int, channels: Int, pixelScale: Int, bin: Int): Long
+  @native def daisyExtract(ctx: Long, grayImages: Long, xDim: Int, yDim: Int, daisyT: Int, daisyQ: Int, daisyR: Int, daisyH: Int,
+      pixelBorder: Int, stride: Int): Long
 
   @native def modelFromHost(ctx: Long, xs: Array[Array[Double]], blockSize: Int, k: Long, b: Array[Double],
       means: Array[Array[Double]]): Long
