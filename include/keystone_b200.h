@@ -294,6 +294,36 @@ KS_API int32_t ks_lbfgs_fit(int64_t ctx, int64_t features, int64_t x_in, const i
                             int32_t fit_intercept, int32_t num_corrections, double convergence_tol, int32_t num_iterations,
                             double reg_param, int32_t precision_mode, int64_t* out_model);
 
+/* ---- sparse matrices and SparseLBFGSwithL2 (DESIGN.md section 20) ---------------------------------------------------------------
+ * A rank's rows of a row-sharded sparse matrix (the reference's RDD[SparseVector[Double]], K/nodes/learning/LBFGS.scala:208-281).
+ * Sparse handles are typed: passing one where a dense matrix handle is expected, or the reverse, returns KS_ERR_HANDLE. */
+/* CSR upload of this rank's n_rows rows: indptr (n_rows + 1), indices and values (indptr[n_rows] each), borrowed for the call.
+ * Stored as fp64 values, int32 column indices and int64 offsets, plus a CSC copy of the same entries built on the device (a stable
+ * radix sort: rows ascend within a column) and work tables that cut long rows and columns into chunks of bounded length.
+ * Unsorted indices within a row and repeated (row, column) entries are legal; every entry contributes its own product, so repeated
+ * entries add up (Breeze's SparseVector built with repeated keys).  Empty rows and n_rows = 0 are legal.  KS_ERR_INVALID with a
+ * message: indptr[0] != 0, a decreasing indptr, an index outside [0, n_cols), a non-finite value, n_cols outside [1, INT32_MAX],
+ * n_rows outside [0, INT32_MAX]. */
+KS_API int32_t ks_sparse_from_host_csr(int64_t ctx, const int64_t* indptr, const int32_t* indices, const double* values, int64_t n_rows,
+                                       int64_t n_cols, int64_t* out_s);
+KS_API int32_t ks_sparse_shape(int64_t ctx, int64_t s, int64_t* n_rows, int64_t* n_cols, int64_t* nnz);
+KS_API int32_t ks_sparse_destroy(int64_t ctx, int64_t s);
+/* Densify (K/nodes/util/Densify.scala): a new n_rows x n_cols fp32 matrix; repeated entries are summed in fp64 in upload order and
+ * rounded once. */
+KS_API int32_t ks_sparse_densify(int64_t ctx, int64_t s, int64_t* out_m);
+/* SparseLBFGSwithL2(LeastSquaresSparseGradient, fitIntercept, numCorrections, convergenceTol, numIterations, regParam).fit
+ * (K/nodes/learning/LBFGS.scala:208-262): no centring; with fit_intercept the data gets an implicit column of ones, and the fit
+ * minimises f = |[A 1][W; b] - Y|^2 / (2N) + reg_param / 2 |[W; b]|^2 (the bias is regularised in f and in g) from zero by the
+ * recursion, exact step and stop rules of ks_lbfgs_fit, all in fp64; labels are the fp32 matrix of this rank's rows.  Returns an
+ * ordinary model handle, W in feature blocks of min(d, 4096) rows, b as the intercept (fit_intercept = 0: W alone), no feature
+ * means.  Both products are gathers in a fixed summation order: one rank fitting the same input twice gets bit-identical models,
+ * and every rank ends with the same bits.  ks_last_fit_stats_json adds solver "sparse_lbfgs" and the global nnz.  Collective. */
+KS_API int32_t ks_sparse_lbfgs_fit(int64_t ctx, int64_t s, int64_t labels, int32_t fit_intercept, int32_t num_corrections,
+                                   double convergence_tol, int32_t num_iterations, double reg_param, int64_t* out_model);
+/* SparseLinearMapper.apply (K/nodes/learning/SparseLinearMapper.scala): A W + b over the CSR rows of s in fp64, rounded once into a
+ * new N x k fp32 matrix.  KS_ERR_INVALID for a model with feature means, a kernel model, or n_cols != the model's d. */
+KS_API int32_t ks_model_apply_sparse(int64_t ctx, int64_t model, int64_t s, int64_t* out_predictions);
+
 /* ---- covariance-based transforms (DESIGN.md section 15) -------------------------------------
  * Every product of these fits runs in fp64 on the DMMA tensor core; they take no precision mode.  The fitted objects are ordinary
  * model handles (apply, save / load, host views): apply runs in the context's precision like every model.  x: this rank's rows

@@ -159,6 +159,36 @@ JFN(jlong, lbfgsFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong xIn,
                                   numIterations, regParam, precisionMode, &h);
   return ok(env, ctx, rc) ? h : 0;
 }
+// ---- sparse matrices and SparseLBFGSwithL2 (DESIGN.md section 20)
+JFN(jlong, sparseFromHostCsr)(JNIEnv* env, jobject, jlong ctx, jlongArray indptr, jintArray indices, jdoubleArray values, jlong nCols) {
+  int64_t h = 0;
+  const jsize nRows = env->GetArrayLength(indptr) - 1;
+  const jsize nnz = env->GetArrayLength(indices);
+  jlong* ip = env->GetLongArrayElements(indptr, nullptr);
+  jint* ix = nnz ? env->GetIntArrayElements(indices, nullptr) : nullptr;
+  jdouble* v = nnz ? env->GetDoubleArrayElements(values, nullptr) : nullptr;
+  const int32_t rc = ks_sparse_from_host_csr(ctx, reinterpret_cast<const int64_t*>(ip), reinterpret_cast<const int32_t*>(ix), v, nRows,
+                                             nCols, &h);
+  if (v) env->ReleaseDoubleArrayElements(values, v, JNI_ABORT);
+  if (ix) env->ReleaseIntArrayElements(indices, ix, JNI_ABORT);
+  env->ReleaseLongArrayElements(indptr, ip, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(void, sparseDestroy)(JNIEnv*, jobject, jlong ctx, jlong s) { ks_sparse_destroy(ctx, s); }
+JFN(jlong, sparseDensify)(JNIEnv* env, jobject, jlong ctx, jlong s) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_sparse_densify(ctx, s, &h)) ? h : 0;
+}
+JFN(jlong, sparseLbfgsFit)(JNIEnv* env, jobject, jlong ctx, jlong s, jlong labels, jboolean fitIntercept, jint numCorrections,
+                           jdouble convergenceTol, jint numIterations, jdouble regParam) {
+  int64_t h = 0;
+  const int32_t rc = ks_sparse_lbfgs_fit(ctx, s, labels, fitIntercept ? 1 : 0, numCorrections, convergenceTol, numIterations, regParam, &h);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, modelApplySparse)(JNIEnv* env, jobject, jlong ctx, jlong model, jlong s) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_model_apply_sparse(ctx, model, s, &h)) ? h : 0;
+}
 JFN(jlong, linearMapFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong labels, jboolean hasLambda, jdouble lambda) {
   int64_t h = 0;
   return ok(env, ctx, ks_linear_map_fit(ctx, features, labels, hasLambda ? 1 : 0, lambda, &h)) ? h : 0;

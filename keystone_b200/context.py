@@ -136,6 +136,35 @@ class Context:
                                                              C.byref(h)))
         return DeviceMatrix(self, h.value, n_rows, n_cols)
 
+    def sparse(self, obj) -> "SparseMatrix":
+        """This rank's rows of a sparse matrix, uploaded as CSR (``ks_sparse_from_host_csr``).  ``obj`` is anything with ``indptr``,
+        ``indices``, ``data`` and ``shape`` (a scipy CSR matrix qualifies; scipy is not needed), or a tuple
+        ``(indptr, indices, data, n_cols)``.  Repeated (row, column) entries add up; unsorted indices and empty rows are legal."""
+        if isinstance(obj, tuple):
+            if len(obj) != 4:
+                raise KeystoneError(-1, "a sparse tuple is (indptr, indices, data, n_cols)")
+            indptr, indices, data, n_cols = obj
+            n_rows = len(indptr) - 1
+        else:
+            indptr, indices, data = obj.indptr, obj.indices, obj.data
+            n_rows, n_cols = int(obj.shape[0]), int(obj.shape[1])
+        indptr = np.ascontiguousarray(indptr, dtype=np.int64)
+        indices = np.asarray(indices)
+        data = np.ascontiguousarray(data, dtype=np.float64)
+        n_cols = int(n_cols)
+        if indptr.ndim != 1 or indptr.shape[0] != n_rows + 1 or n_rows < 0:
+            raise KeystoneError(-1, "indptr must hold n_rows + 1 offsets")
+        nnz = int(indptr[-1])
+        if indices.shape != (nnz,) or data.shape != (nnz,):
+            raise KeystoneError(-1, f"indptr[n_rows] = {nnz} does not match {indices.shape[0]} indices and {data.shape[0]} values")
+        if nnz and (int(indices.min()) < 0 or int(indices.max()) >= n_cols):   # before the int32 cast, which would wrap them
+            raise KeystoneError(-1, "a column index lies outside [0, n_cols)")
+        indices = np.ascontiguousarray(indices, dtype=np.int32)
+        h = C.c_int64(0)
+        check(self.handle, lib().ks_sparse_from_host_csr(self.handle, indptr.ctypes.data_as(C.c_void_p), indices.ctypes.data_as(C.c_void_p),
+                                                          data.ctypes.data_as(C.c_void_p), n_rows, n_cols, C.byref(h)))
+        return SparseMatrix(self, h.value, n_rows, n_cols, nnz)
+
     def labels_from_classes(self, classes: np.ndarray, num_classes: int) -> "DeviceMatrix":
         cls = np.ascontiguousarray(classes, dtype=np.int32)
         h = C.c_int64(0)
@@ -167,6 +196,29 @@ class DeviceMatrix(Dataset):
     def free(self) -> None:
         if self.handle and self.ctx.handle:
             lib().ks_matrix_destroy(self.ctx.handle, self.handle)
+        self.handle = 0
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class SparseMatrix(Dataset):
+    """This rank's rows of a row-sharded sparse matrix on the device (CSR plus a CSC copy): the stand-in for the reference's
+    ``RDD[SparseVector[Double]]``.  Only the sparse nodes take it; the dense nodes reject it."""
+
+    def __init__(self, ctx: Context, handle: int, rows: int, cols: int, nnz: int):
+        self.ctx, self.handle, self.rows, self.cols, self.nnz = ctx, handle, rows, cols, nnz
+
+    @property
+    def shape(self):
+        return (self.rows, self.cols)
+
+    def free(self) -> None:
+        if self.handle and self.ctx.handle:
+            lib().ks_sparse_destroy(self.ctx.handle, self.handle)
         self.handle = 0
 
     def __del__(self):

@@ -212,6 +212,11 @@ Model& Ctx::model(int64_t h) {
   if (it == models.end()) throw KsError{KS_ERR_HANDLE, "unknown model handle " + std::to_string(h)};
   return *it->second;
 }
+SparseMat& Ctx::sparse(int64_t h) {
+  auto it = sparses.find(h);
+  if (it == sparses.end()) throw KsError{KS_ERR_HANDLE, "unknown sparse matrix handle " + std::to_string(h)};
+  return *it->second;
+}
 int64_t Ctx::add(std::unique_ptr<Matrix> m) {
   const int64_t id = next_id++;
   matrices[id] = std::move(m);
@@ -1522,6 +1527,7 @@ KS_API int32_t ks_ctx_destroy(int64_t ctx) {
   if (c->st4) cudaStreamSynchronize(c->st4);
   if (c->st5) cudaStreamSynchronize(c->st5);
   c->matrices.clear();
+  c->sparses.clear();
   c->rfs.clear();
   c->models.clear();
   c->kernels.clear();
@@ -2030,6 +2036,52 @@ KS_API int32_t ks_lbfgs_fit(int64_t ctx, int64_t features, int64_t x_in, const i
     make_feat_src(c, features, x_in, rfs, n_rfs, src, prec);
     *out_model = fit_lbfgs(c, src, c.matrix(labels), fit_intercept != 0, num_corrections, convergence_tol, num_iterations, reg_param,
                            prec);
+  });
+}
+
+// ---------------------------------------------------------------- sparse matrices, SparseLBFGSwithL2 (sparse.cu, lbfgs.cu)
+KS_API int32_t ks_sparse_from_host_csr(int64_t ctx, const int64_t* indptr, const int32_t* indices, const double* values, int64_t n_rows,
+                                       int64_t n_cols, int64_t* out_s) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_s) throw KsError{KS_ERR_INVALID, "null out_s"};
+    auto s = sparse_from_host_csr(c, indptr, indices, values, n_rows, n_cols);
+    const int64_t id = c.next_id++;
+    c.sparses[id] = std::move(s);
+    *out_s = id;
+  });
+}
+KS_API int32_t ks_sparse_shape(int64_t ctx, int64_t s, int64_t* n_rows, int64_t* n_cols, int64_t* nnz) {
+  return guard(ctx, [&](Ctx& c) {
+    SparseMat& sm = c.sparse(s);
+    if (n_rows) *n_rows = sm.rows;
+    if (n_cols) *n_cols = sm.cols;
+    if (nnz) *nnz = sm.nnz;
+  });
+}
+KS_API int32_t ks_sparse_destroy(int64_t ctx, int64_t s) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!c.sparses.erase(s)) throw KsError{KS_ERR_HANDLE, "unknown sparse matrix handle"};
+  });
+}
+KS_API int32_t ks_sparse_densify(int64_t ctx, int64_t s, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(sparse_densify(c, c.sparse(s)));
+  });
+}
+KS_API int32_t ks_sparse_lbfgs_fit(int64_t ctx, int64_t s, int64_t labels, int32_t fit_intercept, int32_t num_corrections,
+                                   double convergence_tol, int32_t num_iterations, double reg_param, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    SparseMat& sm = c.sparse(s);
+    *out_model = fit_sparse_lbfgs(c, sm, c.matrix(labels), fit_intercept != 0, num_corrections, convergence_tol, num_iterations, reg_param);
+  });
+}
+KS_API int32_t ks_model_apply_sparse(int64_t ctx, int64_t model, int64_t s, int64_t* out_predictions) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_predictions) throw KsError{KS_ERR_INVALID, "null output"};
+    Model& m = c.model(model);
+    *out_predictions = c.add(sparse_model_apply(c, m, c.sparse(s)));
   });
 }
 

@@ -153,6 +153,32 @@ struct Model {  // BlockLinearMapper state (K/nodes/learning/BlockLinearMapper.s
   bool host_valid = false;
 };
 
+// A rank's rows of a sparse matrix (sparse.cu, DESIGN.md section 20): CSR as uploaded and a CSC copy of the same entries (columns
+// in order, rows ascending within a column, repeated entries in upload order), each with a work table that cuts its rows / columns
+// into chunks of at most kSpChunk entries.  A line (row or column) of one chunk is written by that chunk; a longer line's chunks write
+// partials that a second pass adds in chunk order.
+static constexpr int64_t kSpChunk = 256;
+struct SpChunk {
+  int64_t begin, end;  // entry range
+  int64_t part;        // -1: the chunk writes its line; otherwise its partial slot
+  int32_t line, pad;
+};
+struct SpSplit {
+  int64_t first;  // partial slots [first, first + count) of the line, in chunk order
+  int32_t line, count;
+};
+struct SpTable {
+  int64_t n_chunks = 0, n_splits = 0;
+  DevBuf chunks, splits;  // SpChunk[n_chunks], SpSplit[n_splits]
+  int64_t n_parts = 0;
+};
+struct SparseMat {
+  int64_t rows = 0, cols = 0, nnz = 0;
+  DevBuf indptr, indices, values;   // CSR: int64[rows + 1], int32[nnz], fp64[nnz]
+  DevBuf colptr, rowidx, cvalues;   // CSC: int64[cols + 1], int32[nnz], fp64[nnz]
+  SpTable rowt, colt;
+};
+
 struct SolverApi {
   void* lib = nullptr;
   cusolverStatus_t (*Create)(cusolverDnHandle_t*) = nullptr;
@@ -261,6 +287,7 @@ struct Ctx {
   std::unordered_map<int64_t, std::unique_ptr<ConvPool>> convs;
   std::unordered_map<int64_t, std::shared_ptr<GaussKernel>> kernels;
   std::unordered_map<int64_t, std::unique_ptr<Gmm>> gmms;
+  std::unordered_map<int64_t, std::unique_ptr<SparseMat>> sparses;
   std::map<std::vector<int>, std::unique_ptr<DevBuf>> tile_cache;
   // phase timing of the current fit
   struct Span { int phase; cudaEvent_t a, b; int stream; };
@@ -273,6 +300,7 @@ struct Ctx {
   Matrix& matrix(int64_t h);
   CosRF& rf(int64_t h);
   Model& model(int64_t h);
+  SparseMat& sparse(int64_t h);
   int64_t add(std::unique_ptr<Matrix> m);
   int64_t add(std::unique_ptr<Model> m);
   cudaEvent_t get_event();
@@ -448,5 +476,21 @@ struct DaisyShape {
 // validates the parameters (throws KS_ERR_INVALID), including ring samples that leave the image; host only
 DaisyShape daisy_shape(int x_dim, int y_dim, int T, int Q, int R, int H, int border, int stride);
 std::unique_ptr<Matrix> daisy_extract(Ctx& c, Matrix& gray_images, int x_dim, int y_dim, int T, int Q, int R, int H, int border, int stride);
+
+// Sparse matrices (sparse.cu); none of these is collective
+std::unique_ptr<SparseMat> sparse_from_host_csr(Ctx& c, const int64_t* indptr, const int32_t* indices, const double* values, int64_t n_rows,
+                                                int64_t n_cols);
+// out (lines x k, row-major fp64) = A X (transpose = false: lines = rows, X is cols x k) or A^T X (transpose = true: lines = cols,
+// X is rows x k), X row-major with ld k; bias_or_null (k values) is added to every line.  Fixed summation order.
+void sparse_product(Ctx& c, const SparseMat& s, bool transpose, const double* X, int k, const double* bias_or_null, double* out,
+                    cudaStream_t st);
+// Xr[(c0 + r) k + c] = Wj[c b + r]: a column-major b x k block of a model (or of the fit's blocked W / P) into rows [c0, c0 + b) of a
+// row-major operand of the CSR product
+void launch_rows_from_block(Ctx& c, const double* Wj, int64_t b, int k, int64_t c0, double* Xr, cudaStream_t st);
+std::unique_ptr<Matrix> sparse_densify(Ctx& c, const SparseMat& s);
+std::unique_ptr<Matrix> sparse_model_apply(Ctx& c, Model& m, const SparseMat& s);
+// SparseLBFGSwithL2 (lbfgs.cu); collective
+int64_t fit_sparse_lbfgs(Ctx& c, const SparseMat& s, Matrix& Y, bool fit_intercept, int num_corrections, double convergence_tol,
+                         int num_iterations, double reg_param);
 
 }  // namespace ks

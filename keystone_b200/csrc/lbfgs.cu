@@ -15,6 +15,9 @@
 // rank reads the same all-reduced inputs, so every rank computes the same bits and the models are bit-identical.  Not ordered:
 // the split-K reduce-add of the tensor-core products and the column sums of the mean passes, as in the block solver, so one
 // rank's fit repeats only up to rounding from run to run.
+//
+// The sparse fit (SparseLBFGSwithL2, DESIGN.md section 20) at the end of the file drives the same recursion (LbCore) with the fp64
+// gather products of sparse.cu in place of the two GEMMs.
 #include "engine.h"
 #include "operand_split.cuh"
 
@@ -126,22 +129,29 @@ __global__ void lb_end_kernel(double* sc, const double* rr, double inv_n, double
 }
 
 // g_new = -(C cs - delta rsum) / N + lambda W over the blocked flat layout (block j: features [j bs, j bs + b_j), column-major
-// b_j x k at offset j bs k); C is row-major D x ldc (feature, class).  y = g_new - g_old and s . y, y . y when y is given.
+// b_j x k at offset j bs k); C is row-major D x ldc (feature, class), fp32 (dense fit) or fp64 (sparse fit).  Entries past D k
+// (n = D k + k: the sparse fit's bias row) take rsum in place of C.  y = g_new - g_old and s . y, y . y when y is given.
 // part: [0] |g|^2, [1] s . y, [2] y . y, [3] max |g|
-__global__ void __launch_bounds__(kRedThreads) lb_gradient_kernel(const float* __restrict__ C, int64_t ldc, const double* __restrict__ delta,
+template <class CT>
+__global__ void __launch_bounds__(kRedThreads) lb_gradient_kernel(const CT* __restrict__ C, int64_t ldc, const double* __restrict__ delta,
                                                                   const double* __restrict__ rsum, const float* __restrict__ c_scale,
                                                                   const double* __restrict__ W, double* g, double* y,
                                                                   const double* __restrict__ s, double inv_n, double lam, int64_t D,
                                                                   int k, int bs, int64_t n, double* part) {
   const double cs = c_scale ? static_cast<double>(*c_scale) : 1.0;
-  const int64_t blk = static_cast<int64_t>(bs) * k;
+  const int64_t blk = static_cast<int64_t>(bs) * k, dk = D * k;
   double gg = 0.0, sy = 0.0, yy = 0.0, gm = 0.0;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const int64_t j = i / blk, r = i - j * blk;
-    const int64_t bj = min(static_cast<int64_t>(bs), D - j * bs);
-    const int64_t c = r / bj, f = j * bs + (r - c * bj);
-    double v = static_cast<double>(C[f * ldc + c]) * cs;
-    if (delta) v -= delta[f] * rsum[c];
+    double v;
+    if (i < dk) {
+      const int64_t j = i / blk, r = i - j * blk;
+      const int64_t bj = min(static_cast<int64_t>(bs), D - j * bs);
+      const int64_t c = r / bj, f = j * bs + (r - c * bj);
+      v = static_cast<double>(C[f * ldc + c]) * cs;
+      if (delta) v -= delta[f] * rsum[c];
+    } else {  // n > D k: the bias row of the implicit ones column (sparse fit), whose product with R is R's column sums
+      v = rsum[i - dk];
+    }
     const double gn = -v * inv_n + lam * W[i];
     if (y) {
       const double yi = gn - g[i];
@@ -274,12 +284,184 @@ __global__ void lb_mean_shift_kernel(const double* __restrict__ fsum, double inv
   delta[i] = m - static_cast<double>(s);
 }
 
-// ------------------------------------------------------------------------------------ the fit
-int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, double tol, int num_iter, double lam, int precision) {
+// |Q|^2 per CTA into part[block] over a dense fp64 vector (the sparse fit's Q, N x k row-major)
+__global__ void __launch_bounds__(kRedThreads) lb_sumsq_f64_kernel(const double* __restrict__ Q, int64_t total, double* part) {
+  double a = 0.0;
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total; i += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    a = fma(Q[i], Q[i], a);
+  const double s = lb_block_reduce(a, 0);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+
+// ------------------------------------------------------------------------------------ the recursion shared by both fits
+// The fp64 state of an L-BFGS least-squares fit over a flat vector of n unknowns and everything that does not touch the data:
+// the two-loop direction, the exact step, the new gradient from the all-reduced C = A^T R, and the host's stop rules.  The
+// dense fit (fit_lbfgs) and the sparse fit (fit_sparse_lbfgs) supply the products A P and A^T R around it.
+struct LbCore {
+  Ctx& c;
+  cudaStream_t st;
+  int64_t n;
+  int m;
+  double inv_n, lam;
+  DevBuf W, g, P, hist, sc, part;
+  std::deque<int> order;  // history slots, oldest first
+  std::vector<double> losses;
+  int iterations = 0;
+  std::string stop = "max_iterations";
+  double host_sc[kScHost];
+
+  LbCore(Ctx& c_, int64_t n_, int m_, double inv_n_, double lam_) : c(c_), st(c_.st), n(n_), m(m_), inv_n(inv_n_), lam(lam_) {
+    W.alloc(sizeof(double) * n);
+    g.alloc(sizeof(double) * n);
+    P.alloc(sizeof(double) * n);
+    hist.alloc(sizeof(double) * 2 * static_cast<size_t>(m) * n);  // S slots [0, m), Y slots [m, 2m)
+    sc.alloc(sizeof(double) * (SC_HIST + 3 * m));
+    part.alloc(sizeof(double) * 4 * kRedBlocks);
+    KS_CUDA(cudaMemsetAsync(W.p, 0, W.bytes, st));
+    KS_CUDA(cudaMemsetAsync(sc.p, 0, sc.bytes, st));
+  }
+  double* S_slot(int h) { return hist.as<double>() + static_cast<size_t>(h) * n; }
+  double* Y_slot(int h) { return hist.as<double>() + static_cast<size_t>(m + h) * n; }
+  double* scp(int slot) { return sc.as<double>() + slot; }
+  static int a_of(int h) { return SC_HIST + 3 * h; }
+  static int cf_of(int h) { return SC_HIST + 3 * h + 1; }
+  static int rho_of(int h) { return SC_HIST + 3 * h + 2; }
+  void finish(const double* p, int nparts, int op, int slot, const double* base = nullptr, const double* scale = nullptr, double mul = 1.0) {
+    lb_finish_kernel<<<1, kRedThreads, 0, st>>>(p, nparts, op, sc.as<double>() + slot, base, scale, mul);
+    c.launches += 1;
+  }
+  void lin(double* out, LbTerm t0, LbTerm t1, const double* gscale, int ndots, const double* w0, const double* w1) {
+    lb_lin_dot_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(out, t0, t1, gscale, ndots, w0, w1, n, part.as<double>());
+    c.launches += 1;
+  }
+
+  // g = -(C - delta rsum) / N + lambda W (C = A^T R with R = Y - A W, all-reduced); with slot h >= 0 also y_h = g_new - g_old,
+  // s_h . y_h, y_h . y_h; then the loss from rr = |R|^2
+  template <class CT>
+  void new_gradient(const CT* C, int64_t ldc, const double* delta, const double* rsum, const float* c_scale, int64_t D, int k, int bs,
+                    const double* rr, int h) {
+    c.span_begin(PH_SOLVE);
+    lb_gradient_kernel<CT><<<kRedBlocks, kRedThreads, 0, st>>>(C, ldc, delta, rsum, c_scale, W.as<double>(), g.as<double>(),
+                                                               h >= 0 ? Y_slot(h) : nullptr, h >= 0 ? S_slot(h) : nullptr, inv_n, lam, D,
+                                                               k, bs, n, part.as<double>());
+    c.launches += 1;
+    finish(part.as<double>(), kRedBlocks, 0, SC_GG);
+    if (h >= 0) {
+      finish(part.as<double>() + kRedBlocks, kRedBlocks, 0, SC_SY);
+      finish(part.as<double>() + 2 * kRedBlocks, kRedBlocks, 0, SC_YY);
+    }
+    finish(part.as<double>() + 3 * kRedBlocks, kRedBlocks, 1, SC_GMAX);
+    lb_end_kernel<<<1, 1, 0, st>>>(sc.as<double>(), rr, inv_n, lam, h);
+    c.launches += 1;
+    c.span_end();
+  }
+  void read_scalars() {
+    KS_CUDA(cudaMemcpyAsync(host_sc, sc.p, sizeof(host_sc), cudaMemcpyDeviceToHost, st));
+    KS_CUDA(cudaStreamSynchronize(st));
+  }
+  // after f(W_0), g(W_0): true when there is nothing to do
+  bool start() {
+    read_scalars();
+    losses.assign(1, host_sc[SC_LOSS]);
+    if (host_sc[SC_GMAX] == 0.0) stop = "zero_gradient";
+    return stop == "zero_gradient";
+  }
+  // two-loop recursion over the history into P, <g, P> and |P|^2, then the descent check (P = -g if <g, P> >= 0)
+  void direction() {
+    const int L = static_cast<int>(order.size());
+    if (L == 0) {
+      lin(P.as<double>(), LbTerm{g.as<double>(), nullptr, -1.0}, LbTerm{}, nullptr, 2, g.as<double>(), nullptr);
+    } else {
+      for (int q = L - 1; q >= 0; --q) {  // newest first: a_i = rho_i s_i . q;  q -= a_i y_i
+        const int h = order[q];
+        if (q == L - 1) lin(P.as<double>(), LbTerm{g.as<double>()}, LbTerm{}, nullptr, 1, S_slot(h), nullptr);
+        else lin(P.as<double>(), LbTerm{P.as<double>()}, LbTerm{Y_slot(order[q + 1]), scp(a_of(order[q + 1])), -1.0}, nullptr, 1, S_slot(h), nullptr);
+        finish(part.as<double>(), kRedBlocks, 0, a_of(h), nullptr, scp(rho_of(h)), 1.0);
+      }
+      // r = gamma (q - a_0 y_0); then oldest first: b_i = rho_i y_i . r;  r += (a_i - b_i) s_i
+      for (int q = 0; q < L; ++q) {
+        const int h = order[q];
+        if (q == 0) lin(P.as<double>(), LbTerm{P.as<double>()}, LbTerm{Y_slot(h), scp(a_of(h)), -1.0}, scp(SC_GAMMA), 1, Y_slot(h), nullptr);
+        else lin(P.as<double>(), LbTerm{P.as<double>()}, LbTerm{S_slot(order[q - 1]), scp(cf_of(order[q - 1])), 1.0}, nullptr, 1, Y_slot(h), nullptr);
+        finish(part.as<double>(), kRedBlocks, 0, cf_of(h), scp(a_of(h)), scp(rho_of(h)), -1.0);
+      }
+      const int hn = order[L - 1];  // P = -(r + (a_n - b_n) s_n)
+      lin(P.as<double>(), LbTerm{P.as<double>(), nullptr, -1.0}, LbTerm{S_slot(hn), scp(cf_of(hn)), -1.0}, nullptr, 2, g.as<double>(), nullptr);
+    }
+    finish(part.as<double>(), kRedBlocks, 0, SC_GP);
+    finish(part.as<double>() + kRedBlocks, kRedBlocks, 0, SC_PP);
+    lb_fallback_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(P.as<double>(), g.as<double>(), n, sc.as<double>());
+    lb_fallback_scalars_kernel<<<1, 1, 0, st>>>(sc.as<double>());
+    c.launches += 2;
+  }
+  // after the all-reduce of |A P|^2 into SC_QQ: alpha, W += alpha P, |W|^2 and s = alpha P into the new history slot (returned)
+  int step() {
+    lb_alpha_kernel<<<1, 1, 0, st>>>(sc.as<double>(), inv_n, lam);
+    c.launches += 1;
+    // the new history slot: the oldest one when the history is full
+    const int h = order.empty() ? 0 : (static_cast<int>(order.size()) == m ? order.front() : (order.back() + 1) % m);
+    lin(W.as<double>(), LbTerm{W.as<double>()}, LbTerm{P.as<double>(), scp(SC_ALPHA), 1.0}, nullptr, 1, nullptr, nullptr);  // W += alpha P
+    finish(part.as<double>(), kRedBlocks, 0, SC_WW);
+    lin(S_slot(h), LbTerm{P.as<double>(), scp(SC_ALPHA), 1.0}, LbTerm{}, nullptr, 0, nullptr, nullptr);  // s = alpha P
+    return h;
+  }
+  // after new_gradient(h) of step t: reads the scalars and applies the stop rules; true ends the fit
+  bool accept(int t, int h, int num_iter, double tol) {
+    read_scalars();
+    if (host_sc[SC_CURV] != 0.0) {  // no step was taken
+      stop = "non_positive_curvature";
+      return true;
+    }
+    iterations = t + 1;
+    const double f = host_sc[SC_LOSS], gmax = host_sc[SC_GMAX];
+    losses.push_back(f);
+    if (host_sc[SC_RESET] != 0.0) order.clear();
+    if (!(host_sc[SC_SY] > 0.0)) {
+      stop = "non_positive_curvature";
+      return true;
+    }
+    if (static_cast<int>(order.size()) == m) order.pop_front();
+    order.push_back(h);
+    if (gmax == 0.0) {
+      stop = "zero_gradient";
+      return true;
+    }
+    if (t + 1 == num_iter) {
+      stop = "max_iterations";
+      return true;
+    }
+    if (tol > 0.0) {
+      const size_t L2 = losses.size();
+      double mx = -INFINITY;
+      for (size_t q = (L2 > 11 ? L2 - 11 : 0); q + 1 < L2; ++q) mx = std::max(mx, losses[q]);
+      if (mx - f <= tol * std::fabs(f)) {
+        stop = "function_values_converged";
+        return true;
+      }
+      if (gmax <= std::max(tol * std::fabs(f), 1e-8)) {
+        stop = "gradient_converged";
+        return true;
+      }
+    }
+    return false;
+  }
+  void history_json(std::ostream& js) const {
+    js << ",\"iterations\":" << iterations << ",\"stop_reason\":\"" << stop << "\",\"loss_history\":[";
+    for (size_t q = 0; q < losses.size(); ++q) js << (q ? "," : "") << losses[q];
+    js << "]";
+  }
+};
+
+static void check_lbfgs_args(int m, double tol, int num_iter, double lam) {
   if (m < 1) throw KsError{KS_ERR_INVALID, "numCorrections must be >= 1"};
   if (num_iter < 1) throw KsError{KS_ERR_INVALID, "numIterations must be >= 1"};
   if (!(lam >= 0.0) || !std::isfinite(lam)) throw KsError{KS_ERR_INVALID, "regParam must be finite and >= 0"};
   if (!(tol >= 0.0) || !std::isfinite(tol)) throw KsError{KS_ERR_INVALID, "convergenceTol must be finite and >= 0"};
+}
+
+// ------------------------------------------------------------------------------------ the fit
+int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, double tol, int num_iter, double lam, int precision) {
+  check_lbfgs_args(m, tol, num_iter, lam);
   if (Y.rows != src.n_rows) throw KsError{KS_ERR_INVALID, "features and labels have different row counts"};
   const int64_t n_loc = Y.rows, D = src.D;
   const int k = static_cast<int>(Y.cols);
@@ -323,19 +505,14 @@ int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, do
   const double inv_n = 1.0 / n_total;
 
   // ---- workspace (every buffer from the pool; an exception returns all of it, the model is only created at the end)
-  DevBuf ymean, W, g, P, hist, sc, part, rpart, cpart, Cbuf, red64, shift, delta, mean, fsum, R, Q, r_op, r_lo, scales, samp;
+  DevBuf ymean, rpart, cpart, Cbuf, red64, shift, delta, mean, fsum, R, Q, r_op, r_lo, scales, samp;
   DevBuf slab, slab_lo, sf32, bop, bop_lo, cbias;
   ymean.alloc(sizeof(double) * k);
   launch_scale_f64(ysum.as<double>(), inv_n, nullptr, ymean.as<double>(), k, st);
   c.launches += 1;
-  W.alloc(sizeof(double) * n);
-  g.alloc(sizeof(double) * n);
-  P.alloc(sizeof(double) * n);
-  hist.alloc(sizeof(double) * 2 * static_cast<size_t>(m) * n);  // S slots [0, m), Y slots [m, 2m)
-  auto S_slot = [&](int h) { return hist.as<double>() + static_cast<size_t>(h) * n; };
-  auto Y_slot = [&](int h) { return hist.as<double>() + static_cast<size_t>(m + h) * n; };
-  sc.alloc(sizeof(double) * (SC_HIST + 3 * m));
-  part.alloc(sizeof(double) * 4 * kRedBlocks);
+  LbCore core(c, n, m, inv_n, lam);
+  DevBuf& W = core.W;
+  DevBuf& P = core.P;
   const int64_t rpb = 1024;
   const int res_gx = static_cast<int>((kpad + 127) / 128), res_gy = static_cast<int>((std::max<int64_t>(n_loc, 1) + rpb - 1) / rpb);
   rpart.alloc(sizeof(double) * static_cast<size_t>(res_gx) * res_gy);
@@ -361,8 +538,6 @@ int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, do
   unsigned* maxbits = scales.as<unsigned>();
   const float* rscale = scales.as<float>() + 2;
   float* pscale = scales.as<float>() + 4;
-  KS_CUDA(cudaMemsetAsync(W.p, 0, W.bytes, st));
-  KS_CUDA(cudaMemsetAsync(sc.p, 0, sc.bytes, st));
   KS_CUDA(cudaMemsetAsync(shift.p, 0, shift.bytes, st));
   KS_CUDA(cudaMemsetAsync(mean.p, 0, mean.bytes, st));
   KS_CUDA(cudaMemsetAsync(delta.p, 0, delta.bytes, st));
@@ -436,19 +611,7 @@ int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, do
   const double* dl = fit_intercept ? delta.as<double>() : nullptr;
 
   // ---- the pieces of an iteration
-  auto finish = [&](const double* p, int nparts, int op, int slot, const double* base = nullptr, const double* scale = nullptr,
-                    double mul = 1.0) {
-    lb_finish_kernel<<<1, kRedThreads, 0, st>>>(p, nparts, op, sc.as<double>() + slot, base, scale, mul);
-    c.launches += 1;
-  };
-  auto lin = [&](double* out, LbTerm t0, LbTerm t1, const double* gscale, int ndots, const double* w0, const double* w1) {
-    lb_lin_dot_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(out, t0, t1, gscale, ndots, w0, w1, n, part.as<double>());
-    c.launches += 1;
-  };
-  auto scp = [&](int slot) { return sc.as<double>() + slot; };
-  auto a_of = [&](int h) { return SC_HIST + 3 * h; };
-  auto cf_of = [&](int h) { return SC_HIST + 3 * h + 1; };
-  auto rho_of = [&](int h) { return SC_HIST + 3 * h + 2; };
+  auto scp = [&](int slot) { return core.scp(slot); };
   // R += alpha Q (Q null: R as it is), the operand of the next A^T R, its column sums and |R|^2 (into red64[k], rank-local)
   auto residual = [&](bool with_q) {
     c.span_begin(PH_OTHER);
@@ -504,25 +667,7 @@ int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, do
   };
   // g = A_c^T (A_c W - Y_c) / N + lambda W; with slot h >= 0 also y_h = g_new - g_old, s_h . y_h, y_h . y_h
   auto new_gradient = [&](int h) {
-    c.span_begin(PH_SOLVE);
-    lb_gradient_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(Cm, kpad, dl, red64.as<double>(), f16 ? rscale + 1 : nullptr, W.as<double>(),
-                                                           g.as<double>(), h >= 0 ? Y_slot(h) : nullptr, h >= 0 ? S_slot(h) : nullptr,
-                                                           inv_n, lam, D, k, bs, n, part.as<double>());
-    c.launches += 1;
-    finish(part.as<double>(), kRedBlocks, 0, SC_GG);
-    if (h >= 0) {
-      finish(part.as<double>() + kRedBlocks, kRedBlocks, 0, SC_SY);
-      finish(part.as<double>() + 2 * kRedBlocks, kRedBlocks, 0, SC_YY);
-    }
-    finish(part.as<double>() + 3 * kRedBlocks, kRedBlocks, 1, SC_GMAX);
-    lb_end_kernel<<<1, 1, 0, st>>>(sc.as<double>(), red64.as<double>() + k, inv_n, lam, h);
-    c.launches += 1;
-    c.span_end();
-  };
-  double host_sc[kScHost];
-  auto read_scalars = [&]() {
-    KS_CUDA(cudaMemcpyAsync(host_sc, sc.p, sizeof(host_sc), cudaMemcpyDeviceToHost, st));
-    KS_CUDA(cudaStreamSynchronize(st));
+    core.new_gradient<float>(Cm, kpad, dl, red64.as<double>(), f16 ? rscale + 1 : nullptr, D, k, bs, red64.as<double>() + k, h);
   };
 
   // ---- f(W_0), g(W_0)
@@ -533,42 +678,13 @@ int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, do
     c.launches += 1;
   }
   new_gradient(-1);
-  read_scalars();
-  std::vector<double> losses{host_sc[SC_LOSS]};
-  std::deque<int> order;  // history slots, oldest first
-  int iterations = 0;
-  std::string stop = "max_iterations";
-  if (host_sc[SC_GMAX] == 0.0) stop = "zero_gradient";
+  const bool nothing_to_do = core.start();
   const int64_t pad_cols = kpad;
 
-  for (int t = 0; t < num_iter && stop != "zero_gradient"; ++t) {
+  for (int t = 0; t < num_iter && !nothing_to_do; ++t) {
     // ---- direction: two-loop recursion over the history (P is the work vector), then the descent check
     c.span_begin(PH_SOLVE);
-    const int L = static_cast<int>(order.size());
-    if (L == 0) {
-      lin(P.as<double>(), LbTerm{g.as<double>(), nullptr, -1.0}, LbTerm{}, nullptr, 2, g.as<double>(), nullptr);
-    } else {
-      for (int q = L - 1; q >= 0; --q) {  // newest first: a_i = rho_i s_i . q;  q -= a_i y_i
-        const int h = order[q];
-        if (q == L - 1) lin(P.as<double>(), LbTerm{g.as<double>()}, LbTerm{}, nullptr, 1, S_slot(h), nullptr);
-        else lin(P.as<double>(), LbTerm{P.as<double>()}, LbTerm{Y_slot(order[q + 1]), scp(a_of(order[q + 1])), -1.0}, nullptr, 1, S_slot(h), nullptr);
-        finish(part.as<double>(), kRedBlocks, 0, a_of(h), nullptr, scp(rho_of(h)), 1.0);
-      }
-      // r = gamma (q - a_0 y_0); then oldest first: b_i = rho_i y_i . r;  r += (a_i - b_i) s_i
-      for (int q = 0; q < L; ++q) {
-        const int h = order[q];
-        if (q == 0) lin(P.as<double>(), LbTerm{P.as<double>()}, LbTerm{Y_slot(h), scp(a_of(h)), -1.0}, scp(SC_GAMMA), 1, Y_slot(h), nullptr);
-        else lin(P.as<double>(), LbTerm{P.as<double>()}, LbTerm{S_slot(order[q - 1]), scp(cf_of(order[q - 1])), 1.0}, nullptr, 1, Y_slot(h), nullptr);
-        finish(part.as<double>(), kRedBlocks, 0, cf_of(h), scp(a_of(h)), scp(rho_of(h)), -1.0);
-      }
-      const int hn = order[L - 1];  // P = -(r + (a_n - b_n) s_n)
-      lin(P.as<double>(), LbTerm{P.as<double>(), nullptr, -1.0}, LbTerm{S_slot(hn), scp(cf_of(hn)), -1.0}, nullptr, 2, g.as<double>(), nullptr);
-    }
-    finish(part.as<double>(), kRedBlocks, 0, SC_GP);
-    finish(part.as<double>() + kRedBlocks, kRedBlocks, 0, SC_PP);
-    lb_fallback_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(P.as<double>(), g.as<double>(), n, sc.as<double>());
-    lb_fallback_scalars_kernel<<<1, 1, 0, st>>>(sc.as<double>());
-    c.launches += 2;
+    core.direction();
     // ---- P^T packed per feature block (fp16: one power-of-two scale for all of P), cbias_j = delta_j . P_j
     if (f16) {
       KS_CUDA(cudaMemsetAsync(maxbits + 1, 0, sizeof(unsigned), st));
@@ -617,61 +733,20 @@ int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, do
       c.span_end();
     }
     c.span_begin(PH_OTHER);
-    lb_sumsq_f32_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(Q.as<float>(), n_loc * pad_cols, part.as<double>());
-    finish(part.as<double>(), kRedBlocks, 0, SC_QQ);
+    lb_sumsq_f32_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(Q.as<float>(), n_loc * pad_cols, core.part.as<double>());
+    core.finish(core.part.as<double>(), kRedBlocks, 0, SC_QQ);
     c.launches += 1;
     c.span_end();
     c.span_begin(PH_ALLREDUCE);
     c.allreduce_f64(scp(SC_QQ), 1);
     c.span_end();
     c.span_begin(PH_SOLVE);
-    lb_alpha_kernel<<<1, 1, 0, st>>>(sc.as<double>(), inv_n, lam);
-    c.launches += 1;
-    // ---- the new history slot: the oldest one when the history is full
-    const int h = order.empty() ? 0 : (static_cast<int>(order.size()) == m ? order.front() : (order.back() + 1) % m);
-    lin(W.as<double>(), LbTerm{W.as<double>()}, LbTerm{P.as<double>(), scp(SC_ALPHA), 1.0}, nullptr, 1, nullptr, nullptr);  // W += alpha P
-    finish(part.as<double>(), kRedBlocks, 0, SC_WW);
-    lin(S_slot(h), LbTerm{P.as<double>(), scp(SC_ALPHA), 1.0}, LbTerm{}, nullptr, 0, nullptr, nullptr);  // s = alpha P
+    const int h = core.step();
     c.span_end();
     residual(true);  // R = Y_c - A_c W_new
     gradient_pass(false);
     new_gradient(h);
-    read_scalars();
-    if (host_sc[SC_CURV] != 0.0) {  // no step was taken
-      stop = "non_positive_curvature";
-      break;
-    }
-    iterations = t + 1;
-    const double f = host_sc[SC_LOSS], gmax = host_sc[SC_GMAX];
-    losses.push_back(f);
-    if (host_sc[SC_RESET] != 0.0) order.clear();
-    if (!(host_sc[SC_SY] > 0.0)) {
-      stop = "non_positive_curvature";
-      break;
-    }
-    if (static_cast<int>(order.size()) == m) order.pop_front();
-    order.push_back(h);
-    if (gmax == 0.0) {
-      stop = "zero_gradient";
-      break;
-    }
-    if (t + 1 == num_iter) {
-      stop = "max_iterations";
-      break;
-    }
-    if (tol > 0.0) {
-      const size_t L2 = losses.size();
-      double mx = -INFINITY;
-      for (size_t q = (L2 > 11 ? L2 - 11 : 0); q + 1 < L2; ++q) mx = std::max(mx, losses[q]);
-      if (mx - f <= tol * std::fabs(f)) {
-        stop = "function_values_converged";
-        break;
-      }
-      if (gmax <= std::max(tol * std::fabs(f), 1e-8)) {
-        stop = "gradient_converged";
-        break;
-      }
-    }
+    if (core.accept(t, h, num_iter, tol)) break;
   }
 
   // ---- the model: LinearMapper(W, Some(ybar), Some(mean)) / LinearMapper(W, None, None), W in blocks of bs features
@@ -723,12 +798,221 @@ int64_t fit_lbfgs(Ctx& c, FeatSrc& src, Matrix& Y, bool fit_intercept, int m, do
   js.precision(17);
   js << "{\"solver\":\"lbfgs\",\"n_local\":" << n_loc << ",\"n_total\":" << static_cast<int64_t>(n_total) << ",\"d\":" << D
      << ",\"k\":" << k << ",\"block_size\":" << bs << ",\"num_blocks\":" << nb << ",\"num_corrections\":" << m
-     << ",\"world\":" << c.world << ",\"iterations\":" << iterations << ",\"stop_reason\":\"" << stop << "\",\"loss_history\":[";
-  for (size_t q = 0; q < losses.size(); ++q) js << (q ? "," : "") << losses[q];
-  js << "],\"total_ms\":" << total_ms << ",\"featurize_ms\":" << ms[PH_FEATURIZE] << ",\"gram_ms\":" << ms[PH_GRAM]
+     << ",\"world\":" << c.world;
+  core.history_json(js);
+  js << ",\"total_ms\":" << total_ms << ",\"featurize_ms\":" << ms[PH_FEATURIZE] << ",\"gram_ms\":" << ms[PH_GRAM]
      << ",\"allreduce_ms\":" << ms[PH_ALLREDUCE] << ",\"solve_ms\":" << ms[PH_SOLVE] << ",\"update_ms\":" << ms[PH_UPDATE]
      << ",\"other_ms\":" << ms[PH_OTHER] << ",\"local_flops\":" << flops << ",\"launches\":" << (c.launches - launches0)
      << ",\"mma\":\"" << (x2 ? (f16 ? "f16x2" : "tf32x2") : f16 ? "f16" : "tf32x1") << "\",\"host_ms\":"
+     << std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count() << "}";
+  c.stats_json = js.str();
+  return c.add(std::move(model));
+}
+
+// ------------------------------------------------------------------------------------ the sparse fit
+// SparseLBFGSwithL2 with LeastSquaresSparseGradient (K/nodes/learning/LBFGS.scala:208-281), DESIGN.md section 20: no centring; with
+// an intercept the unknowns are x = [W; b] over [A 1] (the ones column is implicit), and b is regularised in f and in g:
+//   f = |[A 1] x - Y|_F^2 / (2N) + lambda/2 |x|_F^2,   g = [A 1]^T ([A 1] x - Y) / N + lambda x,   x_0 = 0.
+// Everything after the fp32 labels is fp64.  R = Y - [A 1] x (the dense fit's sign), Q = [A 1] P, R -= alpha Q.
+
+// R = Y (x_0 = 0), fp32 labels widened to fp64, row-major ld k
+__global__ void sp_init_residual_kernel(const float* __restrict__ Y, int64_t ldy, int64_t rows, int k, double* __restrict__ R) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= rows * k) return;
+  const int64_t r = i / k;
+  R[i] = static_cast<double>(Y[r * ldy + (i - r * k)]);
+}
+// R -= alpha Q (Q null: R unchanged), then the column sums of R per CTA into cpart[blockIdx.x * k + c] and |R|^2 per CTA into
+// part[blockIdx.x].  CTA = rows [blockIdx.x rpb, +rpb); thread (tx, ty) = threadIdx (% 32, / 32) takes columns c0 + tx, rows
+// ty, ty + 8, ...; both sums are finished in a fixed order.
+__global__ void __launch_bounds__(256) sp_residual_kernel(double* __restrict__ R, const double* __restrict__ Q, const double* __restrict__ alpha,
+                                                          int64_t rows, int k, int64_t rpb, double* __restrict__ cpart,
+                                                          double* __restrict__ part) {
+  __shared__ double red[8][32];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const double a = Q ? *alpha : 0.0;
+  const int64_t r_begin = blockIdx.x * rpb, r_end = min(rows, r_begin + rpb);
+  double sq = 0.0;
+  for (int c0 = 0; c0 < k; c0 += 32) {
+    const int c = c0 + tx;
+    double cs = 0.0;
+    if (c < k) {
+      for (int64_t r = r_begin + ty; r < r_end; r += 8) {
+        double v = R[r * k + c];
+        if (Q) {
+          v -= a * Q[r * k + c];
+          R[r * k + c] = v;
+        }
+        cs += v;
+        sq = fma(v, v, sq);
+      }
+    }
+    red[ty][tx] = cs;
+    __syncthreads();
+    if (ty == 0 && c < k) {
+      double s = 0.0;
+#pragma unroll
+      for (int y = 0; y < 8; ++y) s += red[y][tx];
+      cpart[blockIdx.x * static_cast<int64_t>(k) + c] = s;
+    }
+    __syncthreads();
+  }
+  const double t = lb_block_reduce(sq, 0);
+  if (threadIdx.x == 0) part[blockIdx.x] = t;
+}
+int64_t fit_sparse_lbfgs(Ctx& c, const SparseMat& A, Matrix& Y, bool fit_intercept, int m, double tol, int num_iter, double lam) {
+  check_lbfgs_args(m, tol, num_iter, lam);
+  if (Y.rows != A.rows) throw KsError{KS_ERR_INVALID, "features and labels have different row counts"};
+  const int64_t n_loc = A.rows, D = A.cols;
+  const int k = static_cast<int>(Y.cols);
+  if (k <= 0) throw KsError{KS_ERR_INVALID, "empty problem"};
+  const int bs = static_cast<int>(std::min<int64_t>(D, 4096));  // feature block of the model (as the dense fit's)
+  const int nb = static_cast<int>((D + bs - 1) / bs);
+  const int64_t n = D * k + (fit_intercept ? k : 0);  // [W; b]: W blocked as in the dense fit, then b
+  cudaStream_t st = c.st;
+  const auto host_t0 = std::chrono::steady_clock::now();
+  c.spans.clear();
+  const int64_t launches0 = c.launches;
+  cudaEvent_t ev0 = c.get_event(), ev1 = c.get_event();
+  c.fit_events.push_back(ev0);
+  c.fit_events.push_back(ev1);
+  KS_CUDA(cudaEventRecord(ev0, st));
+
+  // ---- global row and entry counts
+  c.span_begin(PH_OTHER);
+  DevBuf cnt;
+  cnt.alloc(sizeof(double) * 2);
+  launch_set_f64(cnt.as<double>(), static_cast<double>(n_loc), st);
+  launch_set_f64(cnt.as<double>() + 1, static_cast<double>(A.nnz), st);
+  c.launches += 2;
+  c.allreduce_f64(cnt.as<double>(), 2);
+  double tot[2] = {0, 0};
+  KS_CUDA(cudaMemcpyAsync(tot, cnt.p, sizeof(tot), cudaMemcpyDeviceToHost, st));
+  KS_CUDA(cudaStreamSynchronize(st));
+  if (tot[0] < 1) throw KsError{KS_ERR_INVALID, "no training rows"};
+  const double n_total = tot[0], inv_n = 1.0 / n_total;
+
+  LbCore core(c, n, m, inv_n, lam);
+  const int64_t rpb = 1024, nrb = (std::max<int64_t>(n_loc, 1) + rpb - 1) / rpb;
+  DevBuf R, Q, Xr, Cbuf, red64, rpart, cpart;
+  R.alloc(sizeof(double) * static_cast<size_t>(std::max<int64_t>(n_loc, 1)) * k);
+  Q.alloc(R.bytes);
+  Xr.alloc(sizeof(double) * static_cast<size_t>(n));
+  Cbuf.alloc(sizeof(double) * static_cast<size_t>(D) * k);
+  red64.alloc(sizeof(double) * (k + 1));  // column sums of R, then |R|^2
+  rpart.alloc(sizeof(double) * static_cast<size_t>(nrb));
+  cpart.alloc(sizeof(double) * static_cast<size_t>(nrb) * k);
+  if (n_loc > 0) {
+    sp_init_residual_kernel<<<static_cast<unsigned>((n_loc * k + 255) / 256), 256, 0, st>>>(Y.d, Y.ld, n_loc, k, R.as<double>());
+    c.launches += 1;
+  }
+  c.span_end();
+
+  // R -= alpha Q (Q null: R as it is), its column sums and |R|^2 into red64 (rank-local)
+  auto residual = [&](bool with_q) {
+    c.span_begin(PH_OTHER);
+    sp_residual_kernel<<<static_cast<unsigned>(nrb), 256, 0, st>>>(R.as<double>(), with_q ? Q.as<double>() : nullptr, core.scp(SC_ALPHA), n_loc,
+                                                                   k, rpb, cpart.as<double>(), rpart.as<double>());
+    lb_colsum_finish_kernel<<<(k + 127) / 128, 128, 0, st>>>(cpart.as<double>(), static_cast<int>(nrb), k, k, red64.as<double>());
+    lb_finish_kernel<<<1, kRedThreads, 0, st>>>(rpart.as<double>(), static_cast<int>(nrb), 0, red64.as<double>() + k, nullptr, nullptr, 1.0);
+    c.launches += 3;
+    c.span_end();
+  };
+  // C = A^T R, then the all-reduces of C and of (column sums of R, |R|^2)
+  auto gradient_pass = [&]() {
+    c.span_begin(PH_GRAM);
+    KS_CUDA(cudaMemsetAsync(Cbuf.p, 0, Cbuf.bytes, st));
+    sparse_product(c, A, true, R.as<double>(), k, nullptr, Cbuf.as<double>(), st);
+    c.span_end();
+    c.span_begin(PH_ALLREDUCE);
+    c.allreduce_f64(Cbuf.as<double>(), static_cast<size_t>(D) * k);
+    c.allreduce_f64(red64.as<double>(), static_cast<size_t>(k + 1));
+    c.span_end();
+  };
+  auto new_gradient = [&](int h) {
+    core.new_gradient<double>(Cbuf.as<double>(), k, nullptr, red64.as<double>(), nullptr, D, k, bs, red64.as<double>() + k, h);
+  };
+
+  // ---- f(x_0), g(x_0)
+  residual(false);
+  gradient_pass();
+  new_gradient(-1);
+  const bool nothing_to_do = core.start();
+  for (int t = 0; t < num_iter && !nothing_to_do; ++t) {
+    c.span_begin(PH_SOLVE);
+    core.direction();
+    for (int j = 0; j < nb; ++j) {  // P row-major for the gathers: its blocks are the model's layout
+      const int64_t c0 = static_cast<int64_t>(j) * bs;
+      launch_rows_from_block(c, core.P.as<double>() + c0 * k, std::min<int64_t>(D, c0 + bs) - c0, k, c0, Xr.as<double>(), st);
+    }
+    if (fit_intercept)
+      KS_CUDA(cudaMemcpyAsync(Xr.as<double>() + D * k, core.P.as<double>() + D * k, sizeof(double) * k, cudaMemcpyDeviceToDevice, st));
+    c.span_end();
+    // ---- Q = [A 1] P, |Q|^2, alpha
+    c.span_begin(PH_UPDATE);
+    if (n_loc > 0) KS_CUDA(cudaMemsetAsync(Q.p, 0, Q.bytes, st));
+    sparse_product(c, A, false, Xr.as<double>(), k, fit_intercept ? Xr.as<double>() + D * k : nullptr, Q.as<double>(), st);
+    c.span_end();
+    c.span_begin(PH_OTHER);
+    lb_sumsq_f64_kernel<<<kRedBlocks, kRedThreads, 0, st>>>(Q.as<double>(), n_loc * k, core.part.as<double>());
+    core.finish(core.part.as<double>(), kRedBlocks, 0, SC_QQ);
+    c.launches += 1;
+    c.span_end();
+    c.span_begin(PH_ALLREDUCE);
+    c.allreduce_f64(core.scp(SC_QQ), 1);
+    c.span_end();
+    c.span_begin(PH_SOLVE);
+    const int h = core.step();
+    c.span_end();
+    residual(true);
+    gradient_pass();
+    new_gradient(h);
+    if (core.accept(t, h, num_iter, tol)) break;
+  }
+
+  // ---- the model: SparseLinearMapper(W, Some(b)) / SparseLinearMapper(W, None), W in blocks of bs features, no feature means
+  auto model = std::make_unique<Model>();
+  model->block_size = bs;
+  model->k = k;
+  model->has_mean = false;
+  model->has_intercept = fit_intercept;
+  model->intercept.alloc(sizeof(double) * k);
+  if (fit_intercept)
+    KS_CUDA(cudaMemcpyAsync(model->intercept.p, core.W.as<double>() + D * k, sizeof(double) * k, cudaMemcpyDeviceToDevice, st));
+  else
+    KS_CUDA(cudaMemsetAsync(model->intercept.p, 0, sizeof(double) * k, st));
+  for (int j = 0; j < nb; ++j) {
+    const int64_t c0 = static_cast<int64_t>(j) * bs;
+    const int64_t b = std::min<int64_t>(D, c0 + bs) - c0;
+    model->brows.push_back(b);
+    auto Wj = std::make_unique<DevBuf>();
+    Wj->alloc(sizeof(double) * static_cast<size_t>(b) * k);
+    KS_CUDA(cudaMemcpyAsync(Wj->p, core.W.as<double>() + c0 * k, Wj->bytes, cudaMemcpyDeviceToDevice, st));
+    model->W.push_back(std::move(Wj));
+  }
+  if (c.host_mirror) {
+    model_alloc_host(*model);
+    for (int j = 0; j < nb; ++j) model_block_to_host(*model, j, st);
+    model_intercept_to_host(*model, st);
+  }
+  KS_CUDA(cudaEventRecord(ev1, st));
+  c.check_async("SparseLBFGSwithL2.fit");
+  float total_ms = 0;
+  cudaEventElapsedTime(&total_ms, ev0, ev1);
+  double ms[PH_COUNT];
+  c.collect_spans(ms);
+  for (cudaEvent_t e : c.fit_events) c.event_pool.push_back(e);
+  c.fit_events.clear();
+  std::ostringstream js;
+  js.precision(17);
+  js << "{\"solver\":\"sparse_lbfgs\",\"n_local\":" << n_loc << ",\"n_total\":" << static_cast<int64_t>(n_total) << ",\"d\":" << D
+     << ",\"k\":" << k << ",\"nnz_local\":" << A.nnz << ",\"nnz\":" << static_cast<int64_t>(tot[1]) << ",\"fit_intercept\":"
+     << (fit_intercept ? "true" : "false") << ",\"block_size\":" << bs << ",\"num_blocks\":" << nb << ",\"num_corrections\":" << m
+     << ",\"world\":" << c.world;
+  core.history_json(js);
+  js << ",\"total_ms\":" << total_ms << ",\"ap_ms\":" << ms[PH_UPDATE] << ",\"atr_ms\":" << ms[PH_GRAM]
+     << ",\"allreduce_ms\":" << ms[PH_ALLREDUCE] << ",\"solve_ms\":" << ms[PH_SOLVE] << ",\"other_ms\":" << ms[PH_OTHER]
+     << ",\"launches\":" << (c.launches - launches0) << ",\"host_ms\":"
      << std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count() << "}";
   c.stats_json = js.str();
   return c.add(std::move(model));

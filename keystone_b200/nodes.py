@@ -14,6 +14,10 @@ Reference classes (K/ = src/main/scala/keystoneml/):
   LinearMapper / LinearMapEstimator   K/nodes/learning/LinearMapper.scala:18-116
   DenseLBFGSwithL2                    K/nodes/learning/LBFGS.scala:135-192
   LeastSquaresDenseGradient           K/nodes/learning/Gradient.scala:29-53
+  SparseLBFGSwithL2                   K/nodes/learning/LBFGS.scala:208-281
+  LeastSquaresSparseGradient          K/nodes/learning/Gradient.scala
+  SparseLinearMapper                  K/nodes/learning/SparseLinearMapper.scala
+  Densify                             K/nodes/util/Densify.scala
 
 Batches are ``DeviceMatrix`` / ``LazyFeatures`` (this rank's rows); 2-D numpy arrays are uploaded on
 the fly when a ``Context`` was given to the node.  No node computes on the host.
@@ -28,7 +32,7 @@ import numpy as np
 
 from . import _capi
 from ._capi import KeystoneError, check, lib
-from .context import Context, Dataset, DeviceMatrix, LazyFeatures, feature_source_args
+from .context import Context, Dataset, DeviceMatrix, LazyFeatures, SparseMatrix, feature_source_args
 from .workflow import Estimator, LabelEstimator, Transformer, WeightedNode
 
 
@@ -654,15 +658,145 @@ class DenseLBFGSwithL2(LabelEstimator, WeightedNode):
         return self.num_iterations * (max(cpu_weight * flops, mem_weight * bytes_scanned) + network_weight * network)
 
 
+def _as_sparse(ctx: Optional[Context], data) -> SparseMatrix:
+    if isinstance(data, SparseMatrix):
+        return data
+    if isinstance(data, Dataset):
+        raise KeystoneError(-1, f"a sparse node needs a SparseMatrix, not {type(data).__name__}")
+    if ctx is None:
+        raise KeystoneError(-1, "host sparse input needs a Context (pass ctx= to the node)")
+    return ctx.sparse(data)
+
+
+class LeastSquaresSparseGradient:
+    """The least-squares gradient of sparse L-BFGS (K/nodes/learning/Gradient.scala): (A W - Y) and A^T (A W - Y) over sparse rows.
+    A marker: the device computes it inside ``SparseLBFGSwithL2.fit``."""
+
+
+class SparseLinearMapper(LinearMapper):
+    """SparseLinearMapper(x, bOpt) (K/nodes/learning/SparseLinearMapper.scala): x (d x k) and an optional intercept, applied to
+    sparse rows as A x + b; it carries no feature means.  ``SparseLinearMapper(x, b_opt, ctx)`` builds it from host arrays (stored
+    in feature blocks of min(d, 4096) rows, as the fit stores it); ``SparseLinearMapper(ctx, handle)`` wraps a fitted or loaded
+    model handle."""
+
+    def __init__(self, x, b_opt=None, ctx: Optional[Context] = None):
+        if isinstance(x, Context):   # (ctx, handle)
+            super().__init__(x, int(b_opt))
+            return
+        if ctx is None:
+            raise KeystoneError(-1, "SparseLinearMapper from host arrays needs a Context (pass ctx=)")
+        x = np.asfortranarray(np.asarray(x, dtype=np.float64))
+        if x.ndim != 2 or x.shape[0] < 1 or x.shape[1] < 1:
+            raise ValueError("x must be a non-empty d x k matrix")
+        bs = min(x.shape[0], 4096)
+        blocks = [np.asfortranarray(x[i:i + bs]) for i in range(0, x.shape[0], bs)]
+        ptrs = (C.POINTER(C.c_double) * len(blocks))(*[w.ctypes.data_as(C.POINTER(C.c_double)) for w in blocks])
+        rows = (C.c_int64 * len(blocks))(*[w.shape[0] for w in blocks])
+        bb = None if b_opt is None else np.ascontiguousarray(b_opt, dtype=np.float64)
+        if bb is not None and bb.shape != (x.shape[1],):
+            raise ValueError("b_opt must hold k values")
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_model_from_host(ctx.handle, ptrs, rows, len(blocks), x.shape[1],
+                                                    None if bb is None else bb.ctypes.data_as(C.c_void_p), None, bs, C.byref(h)))
+        super().__init__(ctx, h.value)
+
+    def apply(self, data):
+        """A W + b for the rows of a ``SparseMatrix`` (or a host sparse object), fp64 on the device, rounded once to fp32."""
+        sm = _as_sparse(self.ctx, data)
+        h = C.c_int64(0)
+        check(self.ctx.handle, lib().ks_model_apply_sparse(self.ctx.handle, self.handle, sm.handle, C.byref(h)))
+        return DeviceMatrix(self.ctx, h.value, sm.rows, self.k)
+
+
+class Densify(Transformer):
+    """Densify (K/nodes/util/Densify.scala): a ``SparseMatrix`` as a new fp32 ``DeviceMatrix``; repeated entries are summed in fp64
+    and rounded once."""
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx
+
+    def apply(self, data) -> DeviceMatrix:
+        sm = _as_sparse(self.ctx, data)
+        h = C.c_int64(0)
+        check(sm.ctx.handle, lib().ks_sparse_densify(sm.ctx.handle, sm.handle, C.byref(h)))
+        return DeviceMatrix(sm.ctx, h.value, sm.rows, sm.cols)
+
+
+class SparseLBFGSwithL2(LabelEstimator, WeightedNode):
+    """``new SparseLBFGSwithL2(gradient, fitIntercept, numCorrections, convergenceTol, numIterations, regParam, sparseOverhead)``
+    (K/nodes/learning/LBFGS.scala:208-281) on the device, in fp64 throughout.
+
+    The data is not centred.  With ``fit_intercept`` the rows get an implicit column of ones (never stored) and the fit minimises
+    f = |[A 1][W; b] - Y|^2 / (2N) + regParam / 2 |[W; b]|^2 from zero, returning ``SparseLinearMapper(W, b)``; without it, W alone.
+    The bias is regularised in both f and its gradient: the reference's gradient regularises it (LBFGS.scala:117) while its loss
+    leaves it out (:106-113), so this fit converges to the zero of the reference's gradient with the f whose gradient that is.  At
+    regParam = 0 (the default) the two agree.  The direction, exact step and stop rules are those of ``DenseLBFGSwithL2``
+    (DESIGN.md sections 14 and 20); ``loss_history``, ``iterations``, ``stop_reason`` and ``stats`` are set after a fit.  One rank
+    fitting the same input twice gets a bit-identical model."""
+
+    def __init__(self, gradient=None, fit_intercept: bool = True, num_corrections: int = 10, convergence_tol: float = 1e-4,
+                 num_iterations: int = 100, reg_param: float = 0.0, sparse_overhead: float = 8.0, ctx: Optional[Context] = None):
+        gradient = LeastSquaresSparseGradient() if gradient is None else gradient
+        if not isinstance(gradient, LeastSquaresSparseGradient):
+            raise ValueError("SparseLBFGSwithL2 supports LeastSquaresSparseGradient only")
+        if int(num_corrections) < 1:
+            raise ValueError("num_corrections must be >= 1")
+        if int(num_iterations) < 1:
+            raise ValueError("num_iterations must be >= 1")
+        convergence_tol, reg_param = float(convergence_tol), float(reg_param)
+        if not (convergence_tol >= 0.0 and math.isfinite(convergence_tol)):
+            raise ValueError("convergence_tol must be finite and >= 0")
+        if not (reg_param >= 0.0 and math.isfinite(reg_param)):
+            raise ValueError("reg_param must be finite and >= 0")
+        self.gradient, self.fit_intercept = gradient, bool(fit_intercept)
+        self.num_corrections, self.convergence_tol, self.num_iterations = int(num_corrections), convergence_tol, int(num_iterations)
+        self.reg_param, self.sparse_overhead, self.ctx = reg_param, float(sparse_overhead), ctx
+        self.weight = self.num_iterations + 1  # LBFGS.scala:220
+        self.loss_history: Optional[List[float]] = None
+        self.iterations: Optional[int] = None
+        self.stop_reason: Optional[str] = None
+        self.stats: Optional[dict] = None
+
+    def fit(self, data, labels) -> SparseLinearMapper:
+        """Collective with several ranks (data and labels: this rank's rows)."""
+        sm = _as_sparse(self.ctx, data)
+        ctx = sm.ctx
+        lb = _as_dataset(ctx, labels)
+        if not isinstance(lb, DeviceMatrix):
+            raise KeystoneError(-1, "labels must be a DeviceMatrix or a 2-D array")
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_sparse_lbfgs_fit(ctx.handle, sm.handle, lb.handle, 1 if self.fit_intercept else 0, self.num_corrections,
+                                                     self.convergence_tol, self.num_iterations, self.reg_param, C.byref(h)))
+        model = SparseLinearMapper(ctx, h.value)
+        self.stats = ctx.last_fit_stats()
+        self.loss_history = [float(v) for v in self.stats["loss_history"]]
+        self.iterations, self.stop_reason = int(self.stats["iterations"]), self.stats["stop_reason"]
+        return model
+
+    def cost(self, n: int, d: int, k: int, sparsity: float, num_machines: int, cpu_weight: float, mem_weight: float,
+             network_weight: float) -> float:
+        """CostModel.cost (LBFGS.scala:264-280)."""
+        flops = float(n) * sparsity * d * k / num_machines
+        bytes_scanned = float(n) * d * sparsity / num_machines
+        network = 2.0 * d * k * math.log(num_machines) / math.log(2.0)
+        return self.num_iterations * (self.sparse_overhead * max(cpu_weight * flops, mem_weight * bytes_scanned)
+                                      + network_weight * network)
+
+
 class LeastSquaresEstimator(LabelEstimator, WeightedNode):
     """The reference's cost-model-driven solver choice (K/nodes/learning/LeastSquaresEstimator.scala:17-87): the four
     options' ``CostModel.cost`` formulas -- dense L-BFGS (K/nodes/learning/LBFGS.scala:175-191), sparse L-BFGS (:264-280),
     ``BlockLeastSquaresEstimator(1000, 3, lambda)`` (BlockLinearMapper.scala:268-282) and ``LinearMapEstimator(Some(lambda))``
     (LinearMapper.scala:100-115) -- with the reference's empirical weights; ``optimize`` returns the cheapest.
 
-    ``fit`` runs the two direct solvers on the GPU.  When the cost model prefers an L-BFGS option, ``fit`` runs the GPU block
+    ``fit`` runs the two direct solvers on the GPU.  When the cost model prefers dense L-BFGS, ``fit`` runs the GPU block
     solver instead and records both in ``selected`` / ``used``.  ``DenseLBFGSwithL2`` exists on the device too, but this routing
-    is kept until measurements say where it beats the block solver (DESIGN.md section 14)."""
+    is kept until measurements say where it beats the block solver (DESIGN.md section 14).
+
+    A ``SparseMatrix`` input is costed with sparsity = local nnz / (local rows x d).  ``sparse_lbfgs`` runs
+    ``SparseLBFGSwithL2(num_iterations=20, reg_param=lam)`` on it; every other choice densifies it first
+    (LeastSquaresEstimator.scala:44-50): ``exact`` then runs ``LinearMapEstimator``, ``block`` and ``dense_lbfgs`` the block
+    solver."""
 
     def __init__(self, lam: float = 0.0, num_machines: Optional[int] = None, cpu_weight: float = 3.8e-4, mem_weight: float = 2.9e-1,
                  network_weight: float = 1.32, ctx: Optional[Context] = None):
@@ -672,14 +806,6 @@ class LeastSquaresEstimator(LabelEstimator, WeightedNode):
         self.selected: Optional[str] = None
         self.used: Optional[str] = None
 
-    @staticmethod
-    def _sparse_lbfgs_cost(n, d, k, sparsity, m, cw, mw, nw, num_iterations: int = 20, sparse_overhead: float = 8.0):
-        """SparseLBFGSwithL2.cost (LBFGS.scala:264-280)."""
-        flops = float(n) * sparsity * d * k / m
-        bytes_scanned = float(n) * d * sparsity / m
-        network = 2.0 * d * k * math.log(m) / math.log(2.0)
-        return num_iterations * (sparse_overhead * max(cw * flops, mw * bytes_scanned) + nw * network)
-
     def costs(self, n: int, d: int, k: int, sparsity: float, num_machines: int) -> dict:
         cw, mw, nw = self.cpu_weight, self.mem_weight, self.network_weight
         block = BlockLeastSquaresEstimator(1000, 3, self.lam)
@@ -687,7 +813,7 @@ class LeastSquaresEstimator(LabelEstimator, WeightedNode):
         exact_bytes = float(n) * d / num_machines + float(d) * d
         return {
             "dense_lbfgs": DenseLBFGSwithL2(num_iterations=20).cost(n, d, k, sparsity, num_machines, cw, mw, nw),
-            "sparse_lbfgs": self._sparse_lbfgs_cost(n, d, k, sparsity, num_machines, cw, mw, nw),
+            "sparse_lbfgs": SparseLBFGSwithL2(num_iterations=20).cost(n, d, k, sparsity, num_machines, cw, mw, nw),
             "block": block.cost(n, d, k, sparsity, num_machines, cw, mw, nw),
             "exact": max(cw * exact_flops, mw * exact_bytes) + nw * float(d) * (d + k),
         }
@@ -700,6 +826,8 @@ class LeastSquaresEstimator(LabelEstimator, WeightedNode):
         return self.selected
 
     def fit(self, data, labels) -> BlockLinearMapper:
+        if isinstance(data, SparseMatrix):
+            return self._fit_sparse(data, labels)
         ds = _as_dataset(self.ctx, data)
         lb = _as_dataset(ds.ctx, labels)
         n_total = ds.rows * max(1, ds.ctx.world_size)
@@ -709,6 +837,21 @@ class LeastSquaresEstimator(LabelEstimator, WeightedNode):
             return LinearMapEstimator(self.lam, ds.ctx).fit(ds, lb)
         self.used = "block"
         return BlockLeastSquaresEstimator(1000, 3, self.lam, ctx=ds.ctx).fit(ds, lb)
+
+    def _fit_sparse(self, sm: SparseMatrix, labels) -> BlockLinearMapper:
+        lb = _as_dataset(sm.ctx, labels)
+        n_total = sm.rows * max(1, sm.ctx.world_size)
+        sparsity = sm.nnz / max(1, sm.rows * sm.cols)   # from the local shard, as n is
+        choice = self.optimize(n_total, sm.cols, lb.cols, sparsity, self.num_machines or sm.ctx.world_size)
+        if choice == "sparse_lbfgs":
+            self.used = "sparse_lbfgs"
+            return SparseLBFGSwithL2(num_iterations=20, reg_param=self.lam, ctx=sm.ctx).fit(sm, lb)
+        dense = Densify().apply(sm)
+        if choice == "exact":
+            self.used = "exact"
+            return LinearMapEstimator(self.lam, sm.ctx).fit(dense, lb)
+        self.used = "block"
+        return BlockLeastSquaresEstimator(1000, 3, self.lam, ctx=sm.ctx).fit(dense, lb)
 
 
 # ------------------------------------------------------------------------------------------ Gaussian-kernel ridge regression

@@ -34,6 +34,14 @@ class KeystoneB200 extends Serializable {
   @native def linearMapFit(ctx: Long, features: Long, labels: Long, hasLambda: Boolean, lambda: Double): Long
   @native def lbfgsFit(ctx: Long, features: Long, xIn: Long, rfs: Array[Long], labels: Long, fitIntercept: Boolean,
       numCorrections: Int, convergenceTol: Double, numIterations: Int, regParam: Double, precisionMode: Int): Long
+  /** Sparse rows as CSR (indptr: nRows + 1 offsets; indices / values: indptr(nRows) each), their Densify, SparseLBFGSwithL2 and
+   *  SparseLinearMapper.apply (DESIGN.md section 20).  A sparse handle is not a matrix handle. */
+  @native def sparseFromHostCsr(ctx: Long, indptr: Array[Long], indices: Array[Int], values: Array[Double], nCols: Long): Long
+  @native def sparseDestroy(ctx: Long, s: Long): Unit
+  @native def sparseDensify(ctx: Long, s: Long): Long
+  @native def sparseLbfgsFit(ctx: Long, s: Long, labels: Long, fitIntercept: Boolean, numCorrections: Int, convergenceTol: Double,
+      numIterations: Int, regParam: Double): Long
+  @native def modelApplySparse(ctx: Long, model: Long, s: Long): Long
   /** PCA / ZCA / approximate PCA (collective, fp64 on the device); omega is the d x l test matrix, DenseMatrix.data. */
   @native def pcaFit(ctx: Long, x: Long, dims: Int): Long
   @native def zcaFit(ctx: Long, x: Long, eps: Double): Long
