@@ -79,9 +79,7 @@ KS_API int32_t ks_ctx_synchronize(int64_t ctx);
 /* tunables (defaults in brackets): "gram_chunk_rows" [0 = chosen from the local row count], "sample_rows" [16384: rows per rank
  * for the shift estimate of generated features], "precision" [2 = KS_PRECISION_F16X2: what KS_PRECISION_DEFAULT and the entry
  * points without a precision argument use], "proj_f16" [1: fp16 projection operands in fp16 mode], "shard_solve" [1: triangular solves sharded by
- * right-hand-side columns over the ranks], "reserve_sms" [8], "timing" [1], "pipeline" [1: all tensor-core kernels of a fit on
- * one stream, solve / factor chains beside it; 0: the two-stream arrangement of round 1], "host_mirror" [1: fits copy each
- * finished model block into pinned host memory while they run]; "custom_solve" [-1: automatic -- the library's own DMMA
+ * right-hand-side columns over the ranks], "reserve_sms" [8], "host_mirror" [1: fits copy each finished model block into pinned host memory while they run]; "custom_solve" [-1: automatic -- the library's own DMMA
  * multi-right-hand-side triangular solve kernel when a rank solves <= 512 columns (multi-GPU), cusolverDnDpotrs otherwise; 0 / 1 force], "dyn_tiles" [1: the projection kernel draws its tiles from a
  * counter], "lookahead" [0 = automatic: blocks the residual-independent work runs ahead, 1 on one GPU, 2 on several], "solve_lanes" [4: concurrent per-class solves of the weighted solver],
  * "split_chunk_rows" [4096: rows per accumulation chain of the parity mode's Gram launches; the tensor core's accumulation error grows with

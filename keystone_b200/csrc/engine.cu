@@ -238,13 +238,11 @@ cudaEvent_t Ctx::get_event() {
   return e;
 }
 void Ctx::span_begin(int phase, cudaStream_t s) {
-  if (!timing) return;
   Span sp{phase, get_event(), get_event(), s == st2 ? 2 : s == st3 ? 3 : s == st4 ? 4 : s == st5 ? 5 : 1};
   KS_CUDA(cudaEventRecord(sp.a, s ? s : st));
   spans.push_back(sp);
 }
 void Ctx::span_end(cudaStream_t s) {
-  if (!timing) return;
   KS_CUDA(cudaEventRecord(spans.back().b, s ? s : st));
 }
 void Ctx::collect_spans(double out_ms[PH_COUNT]) {
@@ -745,12 +743,11 @@ __global__ void sumsq_f64_kernel(const double* p, int64_t n, double* out) {
 //   solve(j)  rhs, triangular solves, W_j += dW, pack dW               fp64, ~230 small kernels
 //   update(j) R -= S_j dW                                              tensor
 //
-// pipeline 1 (default): ONE stream carries every tensor-core kernel in the order C(j), G(j+1), proj(j+2), update(j); the
-// solve and factor chains run on their own higher-priority streams and hide under G(j+1) + proj(j+2).  Two tensor
-// kernels never share the SMs: each is written to own an SM (one CTA, ~200 KB of shared memory), so running two at once
-// only splits the machine, thrashes L2 and stretches both.
-// pipeline 0: the round-1 arrangement (residual chain on st, look-ahead tensor kernels on st2), kept for A/B runs.
-// Slabs, G and H are triple-buffered; cross-stream dependencies are CUDA events; no host synchronisation inside the loop.
+// ONE stream carries every tensor-core kernel in the order C(t), G(t+LA), update(t), proj(t+LA+1) (LA: the look-ahead in
+// blocks); the solve and factor chains run on their own higher-priority streams and hide under G(t+LA) + proj(t+LA+1).  Two
+// tensor kernels never share the SMs: each is written to own an SM (one CTA, ~200 KB of shared memory), so running two at
+// once only splits the machine, thrashes L2 and stretches both.
+// Slabs, G and H rotate through LA + 2 buffers; cross-stream dependencies are CUDA events; no host synchronisation inside the loop.
 static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double lam, int64_t nf_opt,
                            int precision = KS_PRECISION_TF32) {
   if (bs <= 0 || num_iter < 1) throw KsError{KS_ERR_INVALID, "blockSize must be > 0 and numIter >= 1"};
@@ -764,15 +761,12 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   const int bmax = static_cast<int>(std::min<int64_t>(bs, D));
   const int64_t lds = round_up(bmax, 32);
   const int64_t kpad = round_up(k, 32);
-  const bool serial = c.pipeline != 0;
   // stream roles (see the Ctx comment)
-  cudaStream_t S1 = c.st, S2 = c.st2, S3 = c.st3, S4 = c.st4, S5 = c.st5;
-  cudaStream_t ST = S2;                       // projection + G-Gram (both pipelines)
-  cudaStream_t SR = serial ? S2 : S1;         // C-Gram and update: the residual chain's tensor kernels
-  cudaStream_t SS = S1;                       // solve chain
-  cudaStream_t SF = S3;                       // factor chain
-  cudaStream_t SG = serial ? S4 : S2;         // all-reduce of G
-  ncclComm_t commG = serial ? c.comm3 : c.comm2;
+  cudaStream_t SS = c.st;   // set-up before the loop, then the solve chain
+  cudaStream_t ST = c.st2;  // every tensor-core kernel: projection, G-Gram, C-Gram, update
+  cudaStream_t SF = c.st3;  // factor chain
+  cudaStream_t SG = c.st4;  // all-reduce of G (on comm3)
+  cudaStream_t SH = c.st5;  // copies into the host mirror
   const auto host_t0 = std::chrono::steady_clock::now();
   c.spans.clear();
   const int64_t launches0 = c.launches;
@@ -782,28 +776,28 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     return e;
   };
   cudaEvent_t ev0 = new_event(), ev1 = new_event(), ev_init = new_event();
-  KS_CUDA(cudaStreamSynchronize(S2));
-  KS_CUDA(cudaStreamSynchronize(S3));
-  KS_CUDA(cudaStreamSynchronize(S4));
-  KS_CUDA(cudaStreamSynchronize(S5));
-  KS_CUDA(cudaEventRecord(ev0, S1));
+  KS_CUDA(cudaStreamSynchronize(ST));
+  KS_CUDA(cudaStreamSynchronize(SF));
+  KS_CUDA(cudaStreamSynchronize(SG));
+  KS_CUDA(cudaStreamSynchronize(SH));
+  KS_CUDA(cudaEventRecord(ev0, SS));
 
   // ---- label mean (StandardScaler on labels, BlockLinearMapper.scala:215) + global row count
   DevBuf ysum;  // [k] sums, [k] = local row count
   ysum.alloc(sizeof(double) * (k + 1));
-  KS_CUDA(cudaMemsetAsync(ysum.p, 0, ysum.bytes, S1));
+  KS_CUDA(cudaMemsetAsync(ysum.p, 0, ysum.bytes, SS));
   c.span_begin(PH_OTHER);
-  launch_colsum(Y.d, nullptr, Y.ld, n_loc, k, ysum.as<double>(), S1);
+  launch_colsum(Y.d, nullptr, Y.ld, n_loc, k, ysum.as<double>(), SS);
   c.launches += 1;
   {
     const double nl = static_cast<double>(n_loc);
-    KS_CUDA(cudaMemcpyAsync(ysum.as<double>() + k, &nl, sizeof(double), cudaMemcpyHostToDevice, S1));
-    KS_CUDA(cudaStreamSynchronize(S1));
+    KS_CUDA(cudaMemcpyAsync(ysum.as<double>() + k, &nl, sizeof(double), cudaMemcpyHostToDevice, SS));
+    KS_CUDA(cudaStreamSynchronize(SS));
   }
   c.allreduce_f64(ysum.as<double>(), k + 1);
   double n_total_d = 0;
-  KS_CUDA(cudaMemcpyAsync(&n_total_d, ysum.as<double>() + k, sizeof(double), cudaMemcpyDeviceToHost, S1));
-  KS_CUDA(cudaStreamSynchronize(S1));
+  KS_CUDA(cudaMemcpyAsync(&n_total_d, ysum.as<double>() + k, sizeof(double), cudaMemcpyDeviceToHost, SS));
+  KS_CUDA(cudaStreamSynchronize(SS));
   if (n_total_d < 1) throw KsError{KS_ERR_INVALID, "no training rows"};
   auto model = std::make_unique<Model>();
   model->block_size = bs;
@@ -811,7 +805,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   model->has_mean = true;
   model->has_intercept = true;
   model->intercept.alloc(sizeof(double) * k);
-  scale_f64_to_f32_kernel<<<(k + 255) / 256, 256, 0, S1>>>(ysum.as<double>(), 1.0 / n_total_d, nullptr,
+  scale_f64_to_f32_kernel<<<(k + 255) / 256, 256, 0, SS>>>(ysum.as<double>(), 1.0 / n_total_d, nullptr,
                                                           model->intercept.as<double>(), k);
   c.launches += 1;
   auto block_cols = [&](int j, int64_t* c0) {
@@ -852,7 +846,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   // look-ahead of the residual-independent work (projection, G-Gram, factorisation) over the residual chain, in blocks.  With the
   // rows sharded over GPUs the Cholesky of block t+1 (slower next to tensor kernels than alone) sits in a dependency cycle
   // G(t+1) -> factor(t+1) -> solve(t+1) -> update(t+1) -> ... -> G(t+1+LA): a deeper look-ahead spreads it over more blocks.
-  const int LA = (serial && (c.pipeline == 1 || c.pipeline == 4)) ? (c.lookahead > 0 ? c.lookahead : (c.world > 1 ? 2 : 1)) : 1;
+  const int LA = c.lookahead > 0 ? c.lookahead : (c.world > 1 ? 2 : 1);
   const int NBUF = LA + 2;
   // which kernel performs the triangular solves of the critical chain (Ctx::custom_solve)
   const bool custom_solve = c.custom_solve == 1 || (c.custom_solve < 0 && c.world > 1 && c.shard_solve && k >= c.world &&
@@ -865,7 +859,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   r_f32.alloc(sizeof(float) * static_cast<size_t>(std::max<int64_t>(n_loc, 1) * kpad));
   r_op.alloc(f16 ? r_f32.bytes / 2 : r_f32.bytes);
   if (x2) r_lo.alloc(r_op.bytes);
-  launch_init_residual(Y.d, Y.ld, model->intercept.as<double>(), r_f32.as<float>(), kpad, n_loc, k, S1);
+  launch_init_residual(Y.d, Y.ld, model->intercept.as<double>(), r_f32.as<float>(), kpad, n_loc, k, SS);
   c.launches += 1;
   // scales: [0] max|R0| bits, [1] max|dW| bits (per block), then float pairs {2^e, 2^-e}: [2,3] residual, [4,5] increment
   scales.alloc(sizeof(float) * 8);
@@ -873,10 +867,10 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   const float* rscale = scales.as<float>() + 2;
   float* dwscale = scales.as<float>() + 4;
   if (f16) {
-    KS_CUDA(cudaMemsetAsync(scales.p, 0, scales.bytes, S1));
-    launch_max_abs_f32(r_f32.as<float>(), kpad, n_loc, k, maxbits, S1);
+    KS_CUDA(cudaMemsetAsync(scales.p, 0, scales.bytes, SS));
+    launch_max_abs_f32(r_f32.as<float>(), kpad, n_loc, k, maxbits, SS);
     c.allreduce_max_u32(maxbits, 1);  // every rank must scale its rows of R alike: C is summed over the ranks
-    launch_pow2_scale(maxbits, 4096.f, scales.as<float>() + 2, S1);  // 16x headroom below fp16's 65504 for later residuals
+    launch_pow2_scale(maxbits, 4096.f, scales.as<float>() + 2, SS);  // 16x headroom below fp16's 65504 for later residuals
     c.launches += 2;
   }
   c.span_end();
@@ -911,26 +905,24 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   if (src.F) {
     c.span_begin(PH_FEATURIZE);
     fsum.alloc(sizeof(double) * static_cast<size_t>(src.F->ld));
-    KS_CUDA(cudaMemsetAsync(fsum.p, 0, fsum.bytes, S1));
-    launch_colsum(src.F->d, nullptr, src.F->ld, n_loc, static_cast<int>(src.F->cols), fsum.as<double>(), S1);
+    KS_CUDA(cudaMemsetAsync(fsum.p, 0, fsum.bytes, SS));
+    launch_colsum(src.F->d, nullptr, src.F->ld, n_loc, static_cast<int>(src.F->cols), fsum.as<double>(), SS);
     c.launches += 1;
     c.allreduce_f64(fsum.as<double>(), static_cast<size_t>(src.F->cols));
     c.span_end();
   }
-  KS_CUDA(cudaEventRecord(ev_init, S1));
-  KS_CUDA(cudaStreamWaitEvent(S2, ev_init, 0));
-  KS_CUDA(cudaStreamWaitEvent(S3, ev_init, 0));
+  KS_CUDA(cudaEventRecord(ev_init, SS));
+  KS_CUDA(cudaStreamWaitEvent(ST, ev_init, 0));
+  KS_CUDA(cudaStreamWaitEvent(SF, ev_init, 0));
 
   struct Step { int it, j; };
   std::vector<Step> steps;
   for (int it = 0; it < num_iter; ++it)
     for (int j = 0; j < nb; ++j) steps.push_back({it, j});
   const int T = static_cast<int>(steps.size());
-  std::vector<cudaEvent_t> ev_slab(T), ev_fact(T), ev_upd(T), ev_gdone(T), ev_g(T), ev_c(T), ev_solved(T);
+  std::vector<cudaEvent_t> ev_fact(T), ev_gdone(T), ev_g(T), ev_c(T), ev_solved(T);
   for (int t = 0; t < T; ++t) {
-    ev_slab[t] = new_event();
     ev_fact[t] = new_event();
-    ev_upd[t] = new_event();
     ev_gdone[t] = new_event();
     ev_g[t] = new_event();
     ev_c[t] = new_event();
@@ -1004,7 +996,6 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
       c.launches += 1;
     }
     c.span_end(ST);
-    KS_CUDA(cudaEventRecord(ev_slab[t], ST));
   };
   // ---------------- gram(t): G of step t on ST, its all-reduce on SG, the factorisation on SF
   auto do_gram = [&](int t) {
@@ -1032,11 +1023,11 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     c.span_end(ST);
     KS_CUDA(cudaEventRecord(ev_gdone[t], ST));
     if (c.world > 1) {
-      if (SG != ST) KS_CUDA(cudaStreamWaitEvent(SG, ev_gdone[t], 0));
+      KS_CUDA(cudaStreamWaitEvent(SG, ev_gdone[t], 0));
       c.span_begin(PH_ALLREDUCE, SG);
-      c.allreduce_on(gbuf[buf].p, g_elems * (g_cross ? 2 : 1), false, commG, SG);
-      c.allreduce_on(ssum[buf].p, static_cast<size_t>(b), false, commG, SG);
-      if (x2) c.allreduce_on(dsq[buf].p, static_cast<size_t>(b), true, commG, SG);
+      c.allreduce_on(gbuf[buf].p, g_elems * (g_cross ? 2 : 1), false, c.comm3, SG);
+      c.allreduce_on(ssum[buf].p, static_cast<size_t>(b), false, c.comm3, SG);
+      if (x2) c.allreduce_on(dsq[buf].p, static_cast<size_t>(b), true, c.comm3, SG);
       c.span_end(SG);
       KS_CUDA(cudaEventRecord(ev_g[t], SG));
     } else {
@@ -1076,46 +1067,45 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     KS_CUDA(cudaEventRecord(ev_fact[t], SF));
     flops += static_cast<double>(b) * b * b / 3.0;
   };
-  // ---------------- cgram(t): operand copy of R + C = S^T R on SR
+  // ---------------- cgram(t): operand copy of R + C = S^T R on ST
   auto do_cgram = [&](int t) {
     const int j = steps[t].j, buf = t % NBUF;
     int64_t c0;
     const int b = block_cols(j, &c0);
-    c.span_begin(PH_OTHER, SR);
-    KS_CUDA(cudaMemsetAsync(cm.p, 0, sizeof(float) * c_elems, SR));
-    KS_CUDA(cudaMemsetAsync(rsum.p, 0, rsum.bytes, SR));
-    if (f16) launch_round_colsum16(r_f32.as<float>(), r_op.p, kpad, n_loc, k, rsum.as<double>(), rscale, SR, x2 ? r_lo.p : nullptr,
+    c.span_begin(PH_OTHER, ST);
+    KS_CUDA(cudaMemsetAsync(cm.p, 0, sizeof(float) * c_elems, ST));
+    KS_CUDA(cudaMemsetAsync(rsum.p, 0, rsum.bytes, ST));
+    if (f16) launch_round_colsum16(r_f32.as<float>(), r_op.p, kpad, n_loc, k, rsum.as<double>(), rscale, ST, x2 ? r_lo.p : nullptr,
                                    maxbits + 6);   // scales[6]: fp16 overflow flag of the residual operand
-    else launch_round_colsum(r_f32.as<float>(), r_op.as<float>(), kpad, n_loc, k, rsum.as<double>(), SR, x2 ? r_lo.as<float>() : nullptr);
+    else launch_round_colsum(r_f32.as<float>(), r_op.as<float>(), kpad, n_loc, k, rsum.as<double>(), ST, x2 ? r_lo.as<float>() : nullptr);
     c.launches += 1;
-    c.span_end(SR);
-    if (SR != ST) KS_CUDA(cudaStreamWaitEvent(SR, ev_slab[t], 0));
-    c.span_begin(PH_UPDATE, SR);  // A^T R part of the Gram (accounted with the residual chain)
+    c.span_end(ST);
+    c.span_begin(PH_UPDATE, ST);  // A^T R part of the Gram (accounted with the residual chain)
     if (x2 && f16) {  // one pass: S_hi^T R_hi + S_lo^T R_hi + S_hi^T R_lo
-      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
+      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, ST, f16,
                         x2_chunk, slab_lo[buf].p, r_lo.p);
       flops += 4.0 * n_loc * static_cast<double>(b) * k;
     } else {
-      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
+      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, ST, f16,
                         x2 ? x2_chunk : 0);
     }
     if (x2 && !f16) {  // + S_lo^T R_hi + S_hi^T R_lo, reduce-added into the same C
-      launch_gram_block(c, slab_lo[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
+      launch_gram_block(c, slab_lo[buf].p, lds, n_loc, b, r_op.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, ST, f16,
                         x2_chunk);
-      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_lo.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, SR, f16,
+      launch_gram_block(c, slab[buf].p, lds, n_loc, b, r_lo.p, kpad, k, nullptr, 0, cm.as<float>(), ldc, false, true, ST, f16,
                         x2_chunk);
       flops += 4.0 * n_loc * static_cast<double>(b) * k;
     }
     flops += 2.0 * n_loc * static_cast<double>(b) * k;
-    c.span_end(SR);
-    KS_CUDA(cudaEventRecord(ev_c[t], SR));
+    c.span_end(ST);
+    KS_CUDA(cudaEventRecord(ev_c[t], ST));
   };
   // ---------------- solve(t): all-reduce of C, rhs, triangular solves, W += dW, operand of the update, on SS
   auto do_solve = [&](int t) {
     const int it = steps[t].it, j = steps[t].j, buf = t % NBUF;
     int64_t c0;
     const int b = block_cols(j, &c0);
-    if (SS != SR) KS_CUDA(cudaStreamWaitEvent(SS, ev_c[t], 0));
+    KS_CUDA(cudaStreamWaitEvent(SS, ev_c[t], 0));
     c.span_begin(PH_ALLREDUCE, SS);
     c.allreduce_f32(cm.as<float>(), c_elems);
     c.allreduce_f64(rsum.as<double>(), k);
@@ -1169,103 +1159,69 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     c.span_end(SS);
     KS_CUDA(cudaEventRecord(ev_solved[t], SS));
     if (it == num_iter - 1 && model->host_valid) {  // W_j and mean_j are final: mirror them to the host while the fit goes on
-      KS_CUDA(cudaStreamWaitEvent(S5, ev_solved[t], 0));
-      model_block_to_host(*model, j, S5);
+      KS_CUDA(cudaStreamWaitEvent(SH, ev_solved[t], 0));
+      model_block_to_host(*model, j, SH);
     }
   };
-  // ---------------- update(t): R -= S dW on SR
+  // ---------------- update(t): R -= S dW on ST
   auto do_update = [&](int t) {
     const int j = steps[t].j, buf = t % NBUF;
     int64_t c0;
     const int b = block_cols(j, &c0);
-    if (SR != SS) KS_CUDA(cudaStreamWaitEvent(SR, ev_solved[t], 0));
-    c.span_begin(PH_UPDATE, SR);
+    KS_CUDA(cudaStreamWaitEvent(ST, ev_solved[t], 0));
+    c.span_begin(PH_UPDATE, ST);
     if (x2 && f16) {  // one pass: R -= S_hi dW_hi + S_lo dW_hi + S_hi dW_lo
       launch_update(c, slab[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, cbias.as<float>(), EPI_UPDATE,
-                    /*reduce=*/true, SR, f16, dwscale + 1, slab_lo[buf].p, bop_lo.p);
+                    /*reduce=*/true, ST, f16, dwscale + 1, slab_lo[buf].p, bop_lo.p);
       flops += 4.0 * n_loc * static_cast<double>(b) * k;
     } else {
       launch_update(c, slab[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, cbias.as<float>(),
-                    EPI_UPDATE, /*reduce=*/true, SR, f16, f16 ? dwscale + 1 : nullptr);
+                    EPI_UPDATE, /*reduce=*/true, ST, f16, f16 ? dwscale + 1 : nullptr);
     }
     if (x2 && !f16) {  // - S_lo dW_hi - S_hi dW_lo (the constant delta^T dW is applied once, above)
-      launch_update(c, slab_lo[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, nullptr, EPI_UPDATE, true, SR, f16,
+      launch_update(c, slab_lo[buf].p, lds, n_loc, b, bop.p, lds, k, r_f32.as<float>(), kpad, nullptr, EPI_UPDATE, true, ST, f16,
                     f16 ? dwscale + 1 : nullptr);
-      launch_update(c, slab[buf].p, lds, n_loc, b, bop_lo.p, lds, k, r_f32.as<float>(), kpad, nullptr, EPI_UPDATE, true, SR, f16,
+      launch_update(c, slab[buf].p, lds, n_loc, b, bop_lo.p, lds, k, r_f32.as<float>(), kpad, nullptr, EPI_UPDATE, true, ST, f16,
                     f16 ? dwscale + 1 : nullptr);
       flops += 4.0 * n_loc * static_cast<double>(b) * k;
     }
     flops += 2.0 * n_loc * static_cast<double>(b) * k;
-    c.span_end(SR);
-    KS_CUDA(cudaEventRecord(ev_upd[t], SR));
+    c.span_end(ST);
   };
 
   // Enqueue order: a stream-wait on an event that has not been recorded yet counts as complete, so every wait is enqueued
   // after the corresponding record.
-  if (serial) {
-    // tensor stream (look-ahead LA, LA + 2 buffers): proj(0..LA) G(0..LA-1) | C(t) G(t+LA) update(t) proj(t+LA+1) | ...
-    // (slab (t+LA+1) % (LA+2) was last read by update(t-1), G buffer (t+LA) % (LA+2) by factor(t-2): both precede in stream / event order).  The solve of step t runs beside
-    // G(t+1): its CTAs fit on the SMs next to Gram CTAs (solve_kernels.cu), not next to the register-heavy projection kernel,
-    // which therefore comes after the update (pipeline = 2 puts it before, for A/B runs).
-    for (int t = 0; t < std::min(T, LA + 1); ++t) do_proj(t);
-    for (int t = 0; t < std::min(T, LA); ++t) do_gram(t);
-    for (int t = 0; t < T; ++t) {
-      do_cgram(t);
-      do_solve(t);
-      if (c.pipeline == 1) {  // C(t), G(t+LA), update(t), proj(t+LA+1): the solve of step t runs beside G(t+LA)
-        if (t + LA < T) do_gram(t + LA);
-        do_update(t);
-        if (t + LA + 1 < T) do_proj(t + LA + 1);
-        continue;
-      }
-      if (c.pipeline == 4) {  // C(t), update(t), G(t+LA), proj(t+LA+1): the tensor stream waits for the solve; nothing shares the
-        do_update(t);         // GPU with it except the factor chain of the block ahead
-        if (t + LA < T) do_gram(t + LA);
-        if (t + LA + 1 < T) do_proj(t + LA + 1);
-        continue;
-      }
-      if (c.pipeline == 3) {  // the solve runs beside the projection (persistent kernel that leaves reserve_sms SMs free)
-        if (t + 2 < T) do_proj(t + 2);
-        do_update(t);
-        if (t + 1 < T) do_gram(t + 1);
-        continue;
-      }
-      if (t + 1 < T) do_gram(t + 1);
-      if (c.pipeline == 2 && t + 2 < T) do_proj(t + 2);
-      do_update(t);
-      if (c.pipeline != 2 && t + 2 < T) do_proj(t + 2);
-    }
-  } else {
-    // proj(t) after update(t - NBUF) released its buffers; G + factor of step t+1 after the chain of step t was enqueued
-    for (int t = 0; t < std::min(T, NBUF - 1); ++t) do_proj(t);
-    do_gram(0);
-    for (int t = 0; t < T; ++t) {
-      do_cgram(t);
-      do_solve(t);
-      do_update(t);
-      if (t + 1 < T) do_gram(t + 1);
-      if (t + NBUF - 1 < T) {
-        if (t >= 1) KS_CUDA(cudaStreamWaitEvent(ST, ev_upd[t - 1], 0));  // step t-1 was the last reader of that slab buffer
-        do_proj(t + NBUF - 1);
-      }
-    }
+  // tensor stream (look-ahead LA, LA + 2 buffers): proj(0..LA) G(0..LA-1) | C(t) G(t+LA) update(t) proj(t+LA+1) | ...
+  // Slab (t+LA+1) % (LA+2) was last read by update(t-1), G buffer (t+LA) % (LA+2) by factor(t-2): both precede in stream /
+  // event order.  The solve of step t runs beside G(t+LA): its CTAs fit on the SMs next to Gram CTAs (solve_kernels.cu), not
+  // next to the register-heavy projection kernel, which therefore comes after the update.
+  for (int t = 0; t < std::min(T, LA + 1); ++t) do_proj(t);
+  for (int t = 0; t < std::min(T, LA); ++t) do_gram(t);
+  for (int t = 0; t < T; ++t) {
+    do_cgram(t);
+    do_solve(t);
+    if (t + LA < T) do_gram(t + LA);
+    do_update(t);
+    if (t + LA + 1 < T) do_proj(t + LA + 1);
   }
-  KS_CUDA(cudaStreamWaitEvent(S1, ev_upd[T - 1], 0));
-  KS_CUDA(cudaStreamWaitEvent(S1, ev_fact[T - 1], 0));
+  cudaEvent_t ev_upd = new_event();  // update(T-1): the last kernel on the tensor stream
+  KS_CUDA(cudaEventRecord(ev_upd, ST));
+  KS_CUDA(cudaStreamWaitEvent(SS, ev_upd, 0));
+  KS_CUDA(cudaStreamWaitEvent(SS, ev_fact[T - 1], 0));
   if (model->host_valid) {
-    model_intercept_to_host(*model, S5);
+    model_intercept_to_host(*model, SH);
     cudaEvent_t ev_copy = new_event();
-    KS_CUDA(cudaEventRecord(ev_copy, S5));
-    KS_CUDA(cudaStreamWaitEvent(S1, ev_copy, 0));  // total_ms ends with the whole model on the host
+    KS_CUDA(cudaEventRecord(ev_copy, SH));
+    KS_CUDA(cudaStreamWaitEvent(SS, ev_copy, 0));  // total_ms ends with the whole model on the host
   }
-  KS_CUDA(cudaEventRecord(ev1, S1));
+  KS_CUDA(cudaEventRecord(ev1, SS));
   c.check_async("BlockLeastSquaresEstimator.fit");
   c.check_infos(info_slot);
   if (f16) {  // collective by construction: every rank scales alike, but only some may overflow -> all-reduce the flag first
     c.allreduce_max_u32(maxbits + 6, 1);
     unsigned ovf = 0;
-    KS_CUDA(cudaMemcpyAsync(&ovf, maxbits + 6, sizeof(unsigned), cudaMemcpyDeviceToHost, S1));
-    KS_CUDA(cudaStreamSynchronize(S1));
+    KS_CUDA(cudaMemcpyAsync(&ovf, maxbits + 6, sizeof(unsigned), cudaMemcpyDeviceToHost, SS));
+    KS_CUDA(cudaStreamSynchronize(SS));
     if (ovf)
       throw KsError{KS_ERR_INVALID, "the residual left fp16's range during the fit (it grew more than 16x over the centred labels): "
                                     "use KS_PRECISION_TF32 for this problem"};
@@ -1289,7 +1245,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
      << ",\"gram_ms\":" << ms[PH_GRAM] << ",\"allreduce_ms\":" << ms[PH_ALLREDUCE] << ",\"solve_ms\":" << ms[PH_SOLVE]
      << ",\"update_ms\":" << ms[PH_UPDATE] << ",\"other_ms\":" << ms[PH_OTHER] << ",\"local_flops\":" << flops
      << ",\"launches\":" << (c.launches - launches0) << ",\"mma\":\"" << (x2 ? (f16 ? "f16x2" : "tf32x2") : f16 ? "f16" : "tf32x1")
-     << "\",\"pipeline\":" << c.pipeline << ",\"lookahead\":" << LA << ",\"host_mirror\":" << (model->host_valid ? 1 : 0) << ",\"solve\":\""
+     << "\",\"lookahead\":" << LA << ",\"host_mirror\":" << (model->host_valid ? 1 : 0) << ",\"solve\":\""
      << (custom_solve ? "dmma-kernel" : "potrs") << (shard_solve ? "-column-sharded" : "") << "\",\"host_ms\":"
      << std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count() << "}";
   c.stats_json = js.str();
@@ -1470,19 +1426,6 @@ KS_API int32_t ks_ctx_create(int32_t device_id, int32_t rank, int32_t world_size
     KS_CUDA(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
     const int prio_mid = (prio_greatest < prio_least) ? prio_greatest + 1 : prio_greatest;
     KS_CUDA(cudaStreamCreateWithPriority(&c->st, cudaStreamNonBlocking, prio_greatest));
-    if (const char* e = getenv("KS_GRAM_CHUNK_ROWS")) {
-      const long v = atol(e);
-      if (v >= kGramStageRows) c->gram_chunk_rows = v;
-    }
-    if (const char* e = getenv("KS_SHARD_SOLVE")) c->shard_solve = atoi(e) != 0;
-    if (const char* e = getenv("KS_PROJ_F16")) c->proj_f16 = atoi(e) != 0;
-    if (const char* e = getenv("KS_PRECISION"))
-      c->precision = (atoi(e) == 1 || !strcmp(e, "f16")) ? KS_PRECISION_F16 : (atoi(e) == 2 || !strcmp(e, "f16x2") || !strcmp(e, "parity")) ? KS_PRECISION_F16X2 : KS_PRECISION_TF32;
-    if (const char* e = getenv("KS_CUSTOM_SOLVE")) c->custom_solve = std::max(-1, std::min(1, atoi(e)));
-    if (const char* e = getenv("KS_RESERVE_SMS")) c->reserve_sms = std::max(0, std::min(140, atoi(e)));
-    if (const char* e = getenv("KS_PIPELINE")) c->pipeline = std::max(0, std::min(4, atoi(e)));
-    if (const char* e = getenv("KS_HOST_MIRROR")) c->host_mirror = atoi(e) != 0;
-    if (const char* e = getenv("KS_LOOKAHEAD")) c->lookahead = std::max(0, std::min(6, atoi(e)));
     KS_CUDA(cudaStreamCreateWithPriority(&c->st2, cudaStreamNonBlocking, prio_least));
     KS_CUDA(cudaStreamCreateWithPriority(&c->st3, cudaStreamNonBlocking, prio_mid));
     KS_CUDA(cudaStreamCreateWithPriority(&c->st4, cudaStreamNonBlocking, prio_mid));
@@ -1587,12 +1530,10 @@ KS_API int32_t ks_ctx_set_option(int64_t ctx, const char* name, int64_t value) {
     else if (n == "precision" && (value == KS_PRECISION_TF32 || value == KS_PRECISION_F16 || value == KS_PRECISION_F16X2)) c.precision = static_cast<int>(value);
     else if (n == "custom_solve" && value >= -1 && value <= 1) c.custom_solve = static_cast<int>(value);
     else if (n == "reserve_sms" && value >= 0 && value < c.num_sms) c.reserve_sms = static_cast<int>(value);
-    else if (n == "pipeline" && value >= 0 && value <= 4) c.pipeline = static_cast<int>(value);
     else if (n == "dyn_tiles") c.dyn_tiles = value != 0;
     else if (n == "lookahead" && value >= 0 && value <= 6) c.lookahead = static_cast<int>(value);
     else if (n == "solve_lanes" && value >= 1 && value <= 16) c.solve_lanes = static_cast<int>(value);
     else if (n == "host_mirror") c.host_mirror = value != 0;
-    else if (n == "timing") c.timing = value != 0;
     else throw KsError{KS_ERR_INVALID, "unknown option or bad value: " + n};
   });
 }

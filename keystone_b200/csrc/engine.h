@@ -225,18 +225,16 @@ enum Phase { PH_FEATURIZE = 0, PH_GRAM, PH_ALLREDUCE, PH_SOLVE, PH_UPDATE, PH_OT
 struct Ctx {
   int device = 0, rank = 0, world = 1;
   int num_sms = 132;
-  // Stream roles of the pipelined fit (engine.cu::fit_blockls), pipeline = 1 (default):
+  // Stream roles of the pipelined fit (engine.cu::fit_blockls), LA = look-ahead in blocks:
   //   st  (highest priority) solve chain: all-reduce of C, rhs assembly, triangular solves, operand packing
-  //   st2 (lowest priority)  ALL tensor-core kernels in one order: C(j), G(j+1), proj(j+2), update(j) -- never two at once
-  //   st3 (mid)              factor chain: fp64 system assembly + Cholesky of the block ahead
+  //   st2 (lowest priority)  ALL tensor-core kernels in one order: C(t), G(t+LA), update(t), proj(t+LA+1) -- never two at once
+  //   st3 (mid)              factor chain: fp64 system assembly + Cholesky of the blocks ahead
   //   st4 (mid)              all-reduce of G
   //   st5 (mid)              D2H copies of finished model blocks into the pinned host mirror
-  // pipeline = 0 is the round-1 arrangement (residual chain incl. its tensor kernels on st, look-ahead tensor kernels on st2).
   cudaStream_t st = nullptr, st2 = nullptr, st3 = nullptr, st4 = nullptr, st5 = nullptr;
   ncclComm_t comm = nullptr;   // collectives issued on st
   ncclComm_t comm2 = nullptr;  // collectives issued on st2 (split of comm; falls back to comm)
-  ncclComm_t comm3 = nullptr;  // collectives issued on st4 (pipeline 1: all-reduce of G)
-  int pipeline = 1;
+  ncclComm_t comm3 = nullptr;  // collectives issued on st4 (all-reduce of G)
   int lookahead = 0;    // blocks the projection / G-Gram / factorisation run ahead of the residual chain; 0 = 1 on one GPU, 2 on several
   int host_mirror = 1;  // fits mirror the model into pinned host memory while they run
   int shard_solve = 1;  // world > 1: every rank runs the triangular solves for its k / world right-hand sides only and the
@@ -295,7 +293,6 @@ struct Ctx {
   std::string timeline_json;
   std::vector<Span> spans;
   std::vector<cudaEvent_t> event_pool;
-  bool timing = true;
 
   Matrix& matrix(int64_t h);
   CosRF& rf(int64_t h);

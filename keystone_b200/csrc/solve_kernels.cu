@@ -18,8 +18,6 @@
 //
 // L: column-major n x n (ld = n), lower triangle valid (cusolverDnDpotrf, CUBLAS_FILL_MODE_LOWER).  B: column-major n x k.
 // Dinv: ceil(n / 64) tiles of 64 x 64 doubles, column-major inside a tile, zero above the diagonal and beyond n.
-#include <stdlib.h>
-
 #include "kernels.h"
 
 namespace ks {
@@ -315,13 +313,10 @@ cudaError_t launch_chol_solve(const double* L, const double* Dinv, int n, double
   if (n <= 0 || k <= 0) return cudaSuccess;
   // 16 right-hand sides per CTA halve the L2 traffic for L (every CTA streams the whole factor twice); with few columns (the
   // column-sharded multi-GPU solve) 8 per CTA keep more SMs busy
-  static const int forced_nc = getenv("KS_SOLVE_NC") ? atoi(getenv("KS_SOLVE_NC")) : 0;   // A/B override (8 or 16)
-  static const int forced_cl = getenv("KS_SOLVE_CLUSTER") ? atoi(getenv("KS_SOLVE_CLUSTER")) : -1;   // -1: chosen from k; 0 / 1: off
   // few right-hand sides: clusters of CTAs share one group of 8 columns, so that up to one CTA per SM (132) works whatever k is
   const int groups = (k + 7) / 8;
-  int cl = forced_cl >= 0 ? forced_cl : (groups <= 16 ? 8 : groups <= 33 ? 4 : groups <= 66 ? 2 : 1);
+  const int cl = groups <= 16 ? 8 : groups <= 33 ? 4 : groups <= 66 ? 2 : 1;
   if (cl > 1) {
-    if (cl != 2 && cl != 4 && cl != 8) return cudaErrorInvalidValue;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(static_cast<unsigned>(groups * cl));
     cfg.blockDim = dim3(256);
@@ -336,8 +331,7 @@ cudaError_t launch_chol_solve(const double* L, const double* Dinv, int n, double
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, chol_solve_cluster_kernel, L, Dinv, n, B, k);
   }
-  const bool nc16 = forced_nc ? forced_nc == 16 : k > 8 * 132;
-  if (nc16) chol_solve_kernel<16><<<(k + 15) / 16, 256, 0, st>>>(L, Dinv, n, B, k);
+  if (k > 8 * 132) chol_solve_kernel<16><<<(k + 15) / 16, 256, 0, st>>>(L, Dinv, n, B, k);
   else chol_solve_kernel<8><<<(k + 7) / 8, 256, 0, st>>>(L, Dinv, n, B, k);
   return cudaGetLastError();
 }

@@ -461,12 +461,10 @@ def test_pooled_convolver_normalized_with_whitener_means(ctx):
 
 
 # ------------------------------------------------------------------------------------------ fit arrangements on one GPU
-OPTION_DEFAULTS = {"pipeline": 1, "lookahead": 0, "dyn_tiles": 1, "proj_f16": 1, "custom_solve": -1}
-# options -> the look-ahead the fit reports (only pipelines 1 and 4 read the option; NBUF = lookahead + 2 slab buffers rotate)
+OPTION_DEFAULTS = {"lookahead": 0, "dyn_tiles": 1, "proj_f16": 1, "custom_solve": -1}
+# options -> the look-ahead the fit reports (NBUF = lookahead + 2 slab buffers rotate)
 ARRANGEMENTS = [
-    ({"pipeline": 0}, 1), ({"pipeline": 1, "lookahead": 1}, 1), ({"pipeline": 1, "lookahead": 2}, 2),
-    ({"pipeline": 1, "lookahead": 4}, 4), ({"pipeline": 2, "lookahead": 4}, 1), ({"pipeline": 3}, 1),
-    ({"pipeline": 4, "lookahead": 1}, 1), ({"pipeline": 4, "lookahead": 2}, 2), ({"pipeline": 4, "lookahead": 4}, 4),
+    ({"lookahead": 1}, 1), ({"lookahead": 2}, 2), ({"lookahead": 4}, 4),
     ({"dyn_tiles": 0}, 1), ({"proj_f16": 0}, 1), ({"custom_solve": 1}, 1),
 ]
 
@@ -499,7 +497,7 @@ def test_fit_arrangements(ctx, fit_problem, options, lookahead):
         for iters in (1, 2):   # one sweep, and two with the factors cached
             model = ks.BlockLeastSquaresEstimator(bs, iters, 2.0, precision="f16" if fast else "default").fit(feats, y)
             stats = ctx.last_fit_stats()
-            assert stats["num_blocks"] == 7 and stats["pipeline"] == options.get("pipeline", 1)
+            assert stats["num_blocks"] == 7
             assert stats["lookahead"] == lookahead and stats["mma"] == ("f16" if fast else "f16x2")
             if options.get("custom_solve") == 1:
                 assert stats["solve"].startswith("dmma-kernel")
@@ -509,3 +507,10 @@ def test_fit_arrangements(ctx, fit_problem, options, lookahead):
     finally:
         for name, value in OPTION_DEFAULTS.items():
             ctx.set_option(name, value)
+
+
+def test_removed_fit_options_rejected(ctx):
+    """The fit has one stream arrangement and always times its phases: the options that selected otherwise are unknown."""
+    for name in ("pipeline", "timing"):
+        with pytest.raises(ks.KeystoneError):
+            ctx.set_option(name, 1)

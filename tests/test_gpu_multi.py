@@ -12,10 +12,8 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _worker(rank, world, id_holder, ret, pipeline, precision):
+def _worker(rank, world, id_holder, ret, custom_solve, precision):
     sys.path.insert(0, ROOT)
-    os.environ["KS_PIPELINE"] = str(pipeline)
-    os.environ["KS_CUSTOM_SOLVE"] = "0" if pipeline == 0 else "-1"      # cuSOLVER potrs in the round-1 arrangement, automatic otherwise
     import keystone_b200 as ks
     from oracle import keystone_oracle as ko
     rng = np.random.default_rng(21)
@@ -26,13 +24,14 @@ def _worker(rank, world, id_holder, ret, pipeline, precision):
     params = [ko.cosine_random_features_params(d_in, n_out, 0.2 / 2, rng) for _ in range(2)]
     lo, hi = ks.shard_range(n, rank, world)
     ctx = ks.Context(device=rank, rank=rank, world_size=world, nccl_id=id_holder["id"])
+    ctx.set_option("custom_solve", custom_solve)   # 0: cuSOLVER potrs, -1: automatic (the DMMA kernel at this k)
     x = ctx.matrix(X[lo:hi]); y = ctx.labels_from_classes(cls[lo:hi], k)
     rfs = [ks.CosineRandomFeatures(ctx, W, b) for W, b in params]
     feats = ks.Pipeline.gather(rfs).andThen(ks.VectorCombiner())(x)
     model = ks.BlockLeastSquaresEstimator(n_out, 2, 0.5, precision=precision).fit(feats, y)
     assert ctx.last_fit_stats()["mma"] == {"f16": "f16", "tf32": "tf32x1", "default": "f16x2"}[precision]
-    assert ctx.last_fit_stats()["pipeline"] == pipeline
-    assert ctx.last_fit_stats()["solve"] == ("potrs-column-sharded" if pipeline == 0 else "dmma-kernel-column-sharded")
+    assert ctx.last_fit_stats()["lookahead"] == 2
+    assert ctx.last_fit_stats()["solve"] == ("potrs-column-sharded" if custom_solve == 0 else "dmma-kernel-column-sharded")
     W = np.concatenate(model.xs, 0)
     cost = model.compute_cost(feats, y, 0.5)
     if rank == 0:
@@ -47,16 +46,16 @@ def _worker(rank, world, id_holder, ret, pipeline, precision):
     ctx.close()
 
 
-@pytest.mark.parametrize("pipeline,precision", [(1, "default"), (1, "f16"), (0, "tf32")],
-                         ids=["parity-mode", "fp16-operands", "tf32-two-stream-pipeline"])
-def test_two_rank_fit_matches_oracle(pipeline, precision):
+@pytest.mark.parametrize("custom_solve,precision", [(-1, "default"), (-1, "f16"), (0, "tf32")],
+                         ids=["parity-mode", "fp16-operands", "tf32-potrs-solve"])
+def test_two_rank_fit_matches_oracle(custom_solve, precision):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     import keystone_b200 as ks
     mgr = mp.Manager()
     id_holder = mgr.dict(); ret = mgr.dict()
     id_holder["id"] = ks.Context.new_nccl_id()
-    mp.spawn(_worker, args=(2, id_holder, ret, pipeline, precision), nprocs=2, join=True)
+    mp.spawn(_worker, args=(2, id_holder, ret, custom_solve, precision), nprocs=2, join=True)
     assert ret["rel"] < (1e-4 if precision == "default" else 1.5e-3), ret["rel"]
     assert ret["cost_rel"] < 1e-4 and ret["b_err"] < 1e-6   # computeCost applies the model in the context's (parity) mode
     assert np.array_equal(ret["W0"], ret["W1"])      # redundant solves are bit-identical across ranks

@@ -1,5 +1,5 @@
 """Timing of the triangular-solve step alone (b = 4096): the library's DMMA kernel vs cusolverDnDpotrs, for the right-hand-side
-counts of the 1/2/4/8-GPU column-sharded solve.  KS_SOLVE_NC=8|16 forces the columns per CTA."""
+counts of the 1/2/4/8-GPU column-sharded solve."""
 import ctypes as C
 import json
 import sys
