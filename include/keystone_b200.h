@@ -258,6 +258,46 @@ KS_API int32_t ks_convolver_create(int64_t ctx, const double* filters_colmajor, 
 KS_API int32_t ks_convolver_apply(int64_t ctx, int64_t conv, int64_t images, int32_t pool_stride, int32_t pool_size, double max_val,
                                   double alpha, int64_t* out_features);
 KS_API int32_t ks_convolver_destroy(int64_t ctx, int64_t conv);
+/* The same chain over views of src_x x src_y source images (views as for ks_image_views, each of the Convolver's x_dim x y_dim):
+ * equal to ks_convolver_apply on ks_image_views' output, without materialising it (each image chunk's views are gathered into a
+ * staging buffer).  Unpooled output is bit-identical to that; pooled output, like ks_convolver_apply's, adds the pool sums with fp32
+ * atomics, so it agrees to the rounding of that order. */
+KS_API int32_t ks_convolver_apply_views(int64_t ctx, int64_t conv, int64_t images, int32_t src_x, int32_t src_y, const int32_t* views,
+                                        int64_t n_views, int32_t pool_stride, int32_t pool_size, double max_val, double alpha,
+                                        int64_t* out_features);
+
+/* ---- image views, Stats.normalizeRows, StandardScaler, AugmentedExamplesEvaluator (DESIGN.md section 21) -----------------------
+ * The front end and the test-time augmentation of K/pipelines/images/cifar/RandomPatchCifar{,Augmented}.scala.  Only the scaler fit
+ * is collective. */
+/* Windower, Cropper, RandomPatcher, CenterCornerPatcher and RandomImageTransformer(flipHorizontal) as a table of views of a batch of
+ * x_dim x y_dim x channels images (rows in ImageVectorizer order): views is n_views x 4 int32 (src_row, x0, y0, flip).  Output
+ * n_views x (out_x out_y channels), view v holding ImageUtils.crop(src, x0, y0, x0 + out_x, y0 + out_y), reversed along y
+ * (ImageUtils.flipHorizontal) when flip is 1, as exact copies.  KS_ERR_INVALID: a view crop would reject (outside the image), a
+ * src_row outside the batch, flip outside {0, 1}, out_x or out_y < 1. */
+KS_API int32_t ks_image_views(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, const int32_t* views, int64_t n_views,
+                              int32_t out_x, int32_t out_y, int64_t* out_m);
+/* Stats.normalizeRows(mat, alpha) (K/utils/Stats.scala:112-123): per row, subtract the mean (NaN -> 0) and divide by
+ * sqrt(sample variance + alpha) (NaN -> sqrt(alpha)), in fp64, rounded once to fp32; a new matrix.  alpha must be finite.  (The
+ * L2 NormalizeRows node is ks_matrix_normalize_rows.) */
+KS_API int32_t ks_matrix_stats_normalize_rows(int64_t ctx, int64_t m, double alpha, int64_t* out_m);
+/* StandardScaler(normalizeStdDev, eps).fit (K/nodes/stats/StandardScaler.scala:38-59): fp64 column means of x over all ranks and,
+ * with normalize_std = 1, the unbiased column std (0 for one row), replaced by 1.0 where it is NaN, infinite or below eps.
+ * mean_out / std_out: cols values each (std_out unused when normalize_std = 0).  Column sums run over fixed row chunks added in
+ * order, without float atomics: a refit on the same rows returns identical bits.  KS_ERR_INVALID: no rows on any rank, eps not
+ * finite or < 0, normalize_std outside {0, 1}.  Collective. */
+KS_API int32_t ks_standard_scaler_fit(int64_t ctx, int64_t x, int32_t normalize_std, double eps, double* mean_out, double* std_out);
+/* StandardScalerModel(mean, std).apply: (x - mean) [/ std] in fp64, rounded once to fp32; a new matrix, padding columns zero.
+ * KS_ERR_INVALID for a non-finite mean or a std that is zero or not finite. */
+KS_API int32_t ks_standard_scaler_apply(int64_t ctx, int64_t x, const double* mean, const double* std_or_null, int64_t* out_m);
+/* AugmentedExamplesEvaluator(names, numClasses, policy).evaluate (K/evaluation/AugmentedExamplesEvaluator.scala) on this rank's
+ * score rows (n_views x k, BlockLinearMapper.apply's output): group g is the views rows[group_offsets[g] .. group_offsets[g+1]),
+ * added in that order in fp64 -- policy 0 (average) the scores, divided by the count; policy 1 (borda) each class's rank in the
+ * view's ascending stable sort.  Then the first maximum is the prediction.  labels: n_views class ids indexed by score row.
+ * out_counts: k x k row-major (rows = true class, columns = prediction), as ks_model_confusion_matrix.  KS_ERR_INVALID: rows not a
+ * permutation of the score rows, offsets not strictly increasing from 0 to n_views, a label outside [0, k), views of one group
+ * with different labels, k != the score columns or k > 4096.  Not collective. */
+KS_API int32_t ks_grouped_confusion_matrix(int64_t ctx, int64_t scores, const int64_t* rows, const int64_t* group_offsets, int64_t n_groups,
+                                           const int32_t* labels, int64_t k, int32_t policy, double* out_counts);
 
 /* ---- feature source shared by fit / apply -------------------------------------------------
  * Either `features` (a materialised N x D matrix; VectorSplitter blocks are column ranges of it,

@@ -85,6 +85,12 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_convolver_create", i64, C.c_void_p, i32, i32, i32, i32, i32, C.c_void_p, i32, f64, p_i64)
     sig("ks_convolver_apply", i64, i64, i64, i32, i32, f64, f64, p_i64)
     sig("ks_convolver_destroy", i64, i64)
+    sig("ks_convolver_apply_views", i64, i64, i64, i32, i32, C.c_void_p, i64, i32, i32, f64, f64, p_i64)
+    sig("ks_image_views", i64, i64, i32, i32, i32, C.c_void_p, i64, i32, i32, p_i64)
+    sig("ks_matrix_stats_normalize_rows", i64, i64, f64, p_i64)
+    sig("ks_standard_scaler_fit", i64, i64, i32, f64, C.c_void_p, C.c_void_p)
+    sig("ks_standard_scaler_apply", i64, i64, C.c_void_p, C.c_void_p, p_i64)
+    sig("ks_grouped_confusion_matrix", i64, i64, C.c_void_p, C.c_void_p, i64, C.c_void_p, i64, i32, C.c_void_p)
     sig("ks_padded_fft_create", i64, C.c_void_p, i64, i32, f64, f64, p_i64)
     sig("ks_matrix_map", i64, i64, i32, C.c_void_p, f64, f64, p_i64)
     sig("ks_matrix_normalize_rows", i64, i64, p_i64)

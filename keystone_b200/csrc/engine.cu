@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include <chrono>
+#include <functional>
 #include <mutex>
 #include <sstream>
 
@@ -1832,15 +1833,11 @@ KS_API int32_t ks_convolver_destroy(int64_t ctx, int64_t conv) {
 // pool_size  > 0: Convolver andThen SymmetricRectifier(max_val, alpha) andThen Pooler(stride, pool_size, identity, sum) andThen
 //                 ImageVectorizer, fused -> (n x nPoolsX*nPoolsY*2*n_filters); the convolved maps never reach HBM.
 // Operands: fp16 (context precision F16 / TF32) or split fp16 pairs concatenated along K (F16X2, the default).
-KS_API int32_t ks_convolver_apply(int64_t ctx, int64_t conv, int64_t images, int32_t pool_stride, int32_t pool_size, double max_val,
-                                  double alpha, int64_t* out_features) {
-  return guard(ctx, [&](Ctx& c) {
-    if (!out_features) throw KsError{KS_ERR_INVALID, "null output"};
-    auto it = c.convs.find(conv);
-    if (it == c.convs.end()) throw KsError{KS_ERR_HANDLE, "unknown Convolver handle"};
-    ConvPool& cv = *it->second;
-    Matrix& im = c.matrix(images);
-    if (im.cols != static_cast<int64_t>(cv.x_dim) * cv.y_dim * cv.ch) throw KsError{KS_ERR_INVALID, "image size does not match the Convolver"};
+// This is the image chunk loop of ks_convolver_apply and ks_convolver_apply_views: chunk_images(i0, ni, chunk_rows) returns the
+// images [i0, i0 + ni) as rows of leading dimension ld_img (chunk_rows: the most images any call asks for).
+static std::unique_ptr<Matrix> convolver_run(Ctx& c, ConvPool& cv, int64_t n_images, int64_t ld_img,
+                                             const std::function<const float*(int64_t, int64_t, int64_t)>& chunk_images,
+                                             int32_t pool_stride, int32_t pool_size, double max_val, double alpha) {
     const int rw = cv.x_dim - cv.conv + 1, rh = cv.y_dim - cv.conv + 1, ppi = rw * rh;
     const bool pooled = pool_size > 0;
     int npx = 0, npy = 0;
@@ -1862,17 +1859,17 @@ KS_API int32_t ks_convolver_apply(int64_t ctx, int64_t conv, int64_t images, int
     const int64_t ldp = x2 ? cv.ld3 : cv.ld1;
     const int kdepth = x2 ? 3 * cv.pd : cv.pd;
     const int64_t out_cols = pooled ? static_cast<int64_t>(npx) * npy * 2 * cv.n_filters : static_cast<int64_t>(ppi) * cv.n_filters;
-    auto out = new_matrix(im.rows, out_cols);
+    auto out = new_matrix(n_images, out_cols);
     KS_CUDA(cudaMemsetAsync(out->d, 0, out->buf.bytes, c.st));
     DevBuf maskd, patches;
     maskd.alloc(sizeof(unsigned) * ppi);
     KS_CUDA(cudaMemcpyAsync(maskd.p, mask.data(), sizeof(unsigned) * ppi, cudaMemcpyHostToDevice, c.st));
     // image chunks bound the patch matrix (ppi * ldp * 2 B per image) to ~4 GB
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(im.rows, (int64_t(4) << 30) / (static_cast<int64_t>(ppi) * ldp * 2)));
+    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(n_images, (int64_t(4) << 30) / (static_cast<int64_t>(ppi) * ldp * 2)));
     patches.alloc(2 * static_cast<size_t>(chunk) * ppi * ldp);
-    for (int64_t i0 = 0; i0 < im.rows; i0 += chunk) {
-      const int64_t ni = std::min(chunk, im.rows - i0);
-      launch_im2col_normalize(im.d + i0 * im.ld, im.ld, ni, cv.x_dim, cv.y_dim, cv.ch, cv.conv, cv.normalize, cv.var_constant,
+    for (int64_t i0 = 0; i0 < n_images; i0 += chunk) {
+      const int64_t ni = std::min(chunk, n_images - i0);
+      launch_im2col_normalize(chunk_images(i0, ni, chunk), ld_img, ni, cv.x_dim, cv.y_dim, cv.ch, cv.conv, cv.normalize, cv.var_constant,
                               cv.has_means ? cv.wmeans.as<float>() : nullptr, patches.p, ldp, x2 ? 1 : 0, c.st);
       KmLaunch k;
       const int64_t m_rows = ni * ppi;
@@ -1898,7 +1895,7 @@ KS_API int32_t ks_convolver_apply(int64_t ctx, int64_t conv, int64_t images, int
         k.p.n_pools = npx * npy;
         k.p.pool_alpha = static_cast<float>(alpha);
         k.p.rect_floor = static_cast<float>(max_val);
-        tmap_or_throw(&k.tmOut, out->d, im.rows, std::min<int64_t>(out_cols, 32), out->ld, 32);  // unused by this epilogue
+        tmap_or_throw(&k.tmOut, out->d, n_images, std::min<int64_t>(out_cols, 32), out->ld, 32);  // unused by this epilogue
       } else {
         // the convolved image of image i is rows [i * ppi, (i+1) * ppi) x n_filters of the product: view the output as that matrix
         k.epi = EPI_APPLY;
@@ -1911,7 +1908,46 @@ KS_API int32_t ks_convolver_apply(int64_t ctx, int64_t conv, int64_t images, int
       KS_CUDA(cudaStreamSynchronize(c.st));   // the patch buffer is reused by the next chunk
     }
     c.check_async("Convolver.apply");
-    *out_features = c.add(std::move(out));
+    return out;
+}
+static ConvPool& conv_of(Ctx& c, int64_t conv) {
+  auto it = c.convs.find(conv);
+  if (it == c.convs.end()) throw KsError{KS_ERR_HANDLE, "unknown Convolver handle"};
+  return *it->second;
+}
+KS_API int32_t ks_convolver_apply(int64_t ctx, int64_t conv, int64_t images, int32_t pool_stride, int32_t pool_size, double max_val,
+                                  double alpha, int64_t* out_features) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_features) throw KsError{KS_ERR_INVALID, "null output"};
+    ConvPool& cv = conv_of(c, conv);
+    Matrix& im = c.matrix(images);
+    if (im.cols != static_cast<int64_t>(cv.x_dim) * cv.y_dim * cv.ch) throw KsError{KS_ERR_INVALID, "image size does not match the Convolver"};
+    *out_features = c.add(convolver_run(c, cv, im.rows, im.ld, [&](int64_t i0, int64_t, int64_t) -> const float* { return im.d + i0 * im.ld; },
+                                        pool_stride, pool_size, max_val, alpha));
+  });
+}
+// The Convolver over views of src_x x src_y source images (augment.cu): each chunk's views are gathered into a staging matrix
+// laid out as ks_image_views' output, then the chunk runs as in ks_convolver_apply.  The views are never all materialised.
+KS_API int32_t ks_convolver_apply_views(int64_t ctx, int64_t conv, int64_t images, int32_t src_x, int32_t src_y, const int32_t* views,
+                                        int64_t n_views, int32_t pool_stride, int32_t pool_size, double max_val, double alpha,
+                                        int64_t* out_features) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_features) throw KsError{KS_ERR_INVALID, "null output"};
+    ConvPool& cv = conv_of(c, conv);
+    Matrix& im = c.matrix(images);
+    if (src_x < 1 || src_y < 1 || im.cols != static_cast<int64_t>(src_x) * src_y * cv.ch)
+      throw KsError{KS_ERR_INVALID, "source image size does not match src_x * src_y * the Convolver's channels"};
+    check_views(views, n_views, im.rows, src_x, src_y, cv.x_dim, cv.y_dim);
+    DevBuf dv, stage;
+    dv.alloc(sizeof(int32_t) * 4 * static_cast<size_t>(std::max<int64_t>(n_views, 1)));
+    if (n_views > 0) KS_CUDA(cudaMemcpyAsync(dv.p, views, sizeof(int32_t) * 4 * n_views, cudaMemcpyHostToDevice, c.st));
+    const int64_t ld = round_up(static_cast<int64_t>(cv.x_dim) * cv.y_dim * cv.ch, kPadCols);
+    auto gather = [&](int64_t i0, int64_t ni, int64_t chunk) -> const float* {
+      if (!stage.p) stage.alloc(sizeof(float) * static_cast<size_t>(chunk * ld));
+      launch_image_views(c, im, src_x, cv.ch, dv.as<int32_t>() + 4 * i0, ni, cv.x_dim, cv.y_dim, stage.as<float>(), ld);
+      return stage.as<float>();
+    };
+    *out_features = c.add(convolver_run(c, cv, n_views, ld, gather, pool_stride, pool_size, max_val, alpha));
   });
 }
 
@@ -2157,6 +2193,36 @@ KS_API int32_t ks_matrix_gather_rows(int64_t ctx, int64_t m, const int64_t* rows
   return guard(ctx, [&](Ctx& c) {
     if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
     *out_m = c.add(gather_rows(c, c.matrix(m), rows, n));
+  });
+}
+
+// ---------------------------------------------------------------- image views, normalizeRows, StandardScaler, evaluator (augment.cu)
+KS_API int32_t ks_image_views(int64_t ctx, int64_t images, int32_t x_dim, int32_t y_dim, int32_t channels, const int32_t* views, int64_t n_views,
+                              int32_t out_x, int32_t out_y, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(image_views(c, c.matrix(images), x_dim, y_dim, channels, views, n_views, out_x, out_y));
+  });
+}
+KS_API int32_t ks_matrix_stats_normalize_rows(int64_t ctx, int64_t m, double alpha, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(stats_normalize_rows(c, c.matrix(m), alpha));
+  });
+}
+KS_API int32_t ks_standard_scaler_fit(int64_t ctx, int64_t x, int32_t normalize_std, double eps, double* mean_out, double* std_out) {
+  return guard(ctx, [&](Ctx& c) { standard_scaler_fit(c, c.matrix(x), normalize_std, eps, mean_out, std_out); });
+}
+KS_API int32_t ks_standard_scaler_apply(int64_t ctx, int64_t x, const double* mean, const double* std_or_null, int64_t* out_m) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_m) throw KsError{KS_ERR_INVALID, "null out_m"};
+    *out_m = c.add(standard_scaler_apply(c, c.matrix(x), mean, std_or_null));
+  });
+}
+KS_API int32_t ks_grouped_confusion_matrix(int64_t ctx, int64_t scores, const int64_t* rows, const int64_t* group_offsets, int64_t n_groups,
+                                           const int32_t* labels, int64_t k, int32_t policy, double* out_counts) {
+  return guard(ctx, [&](Ctx& c) {
+    grouped_confusion_matrix(c, c.matrix(scores), rows, group_offsets, n_groups, labels, k, policy, out_counts);
   });
 }
 

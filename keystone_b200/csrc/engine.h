@@ -474,6 +474,20 @@ struct DaisyShape {
 DaisyShape daisy_shape(int x_dim, int y_dim, int T, int Q, int R, int H, int border, int stride);
 std::unique_ptr<Matrix> daisy_extract(Ctx& c, Matrix& gray_images, int x_dim, int y_dim, int T, int Q, int R, int H, int border, int stride);
 
+// Image views, Stats.normalizeRows, StandardScaler and the grouped confusion matrix (augment.cu).  Only the scaler fit is collective.
+// views: n x 4 int32 (src_row, x0, y0, flip); throws KS_ERR_INVALID for a view ImageUtils.crop would reject or a flip outside {0, 1}
+void check_views(const int32_t* views, int64_t n_views, int64_t n_images, int x_dim, int y_dim, int out_x, int out_y);
+// rows [0, n) of out (ld ldo) = the views d_views[0, n) (device, checked) of images, each out_x * out_y * ch values, padding zeroed
+void launch_image_views(Ctx& c, const Matrix& images, int x_dim, int ch, const int32_t* d_views, int64_t n, int out_x, int out_y,
+                        float* out, int64_t ldo);
+std::unique_ptr<Matrix> image_views(Ctx& c, Matrix& images, int x_dim, int y_dim, int ch, const int32_t* views, int64_t n_views, int out_x,
+                                    int out_y);
+std::unique_ptr<Matrix> stats_normalize_rows(Ctx& c, Matrix& in, double alpha);
+void standard_scaler_fit(Ctx& c, Matrix& X, int normalize_std, double eps, double* mean_out, double* std_out);
+std::unique_ptr<Matrix> standard_scaler_apply(Ctx& c, Matrix& X, const double* mean, const double* std_or_null);
+void grouped_confusion_matrix(Ctx& c, Matrix& scores, const int64_t* rows, const int64_t* group_offsets, int64_t n_groups,
+                              const int32_t* labels, int64_t k, int policy, double* out);
+
 // Sparse matrices (sparse.cu); none of these is collective
 std::unique_ptr<SparseMat> sparse_from_host_csr(Ctx& c, const int64_t* indptr, const int32_t* indices, const double* values, int64_t n_rows,
                                                 int64_t n_cols);

@@ -15,7 +15,7 @@ import numpy as np
 
 from ._capi import check, lib
 from .context import feature_source_args
-from .nodes import BlockLinearMapper, _as_dataset
+from .nodes import BlockLinearMapper, _as_dataset, _device_matrix
 
 
 @dataclass(frozen=True)
@@ -115,3 +115,43 @@ class MulticlassClassifierEvaluator:
     @staticmethod
     def from_confusion_matrix(cm: np.ndarray) -> MulticlassMetrics:
         return MulticlassMetrics(cm)
+
+
+AVERAGE, BORDA = "average", "borda"   # AggregationPolicyType (K/evaluation/AugmentedExamplesEvaluator.scala)
+
+
+class AugmentedExamplesEvaluator:
+    """``new AugmentedExamplesEvaluator(names, numClasses, policy)`` (K/evaluation/AugmentedExamplesEvaluator.scala): the views that
+    share a name are one example.  ``average`` adds their scores and divides by the count; ``borda`` adds each class's rank in the
+    view's ascending stable sort (ties go by class index).  The first maximum is the prediction.  Grouping the names is host
+    bookkeeping (a permutation and group offsets); the pass over the (n_views x k) scores and the counts run on the device
+    (``ks_grouped_confusion_matrix``).  Every view of a name must carry the same label, as the reference asserts.  One rank only:
+    the groups must not span ranks."""
+
+    def __init__(self, names, numClasses: int, policy: str = AVERAGE):
+        if policy not in (AVERAGE, BORDA):
+            raise ValueError("policy must be 'average' or 'borda'")
+        self.names, self.num_classes, self.policy = np.asarray(names), int(numClasses), policy
+
+    def groups(self):
+        """(rows, offsets): the view rows of each name, names in order of first appearance, views in their order."""
+        _, first, inv = np.unique(self.names, return_index=True, return_inverse=True)
+        rank = np.empty(first.size, dtype=np.int64)
+        rank[np.argsort(first, kind="stable")] = np.arange(first.size)
+        g = rank[inv.reshape(-1)]
+        rows = np.argsort(g, kind="stable").astype(np.int64)
+        offsets = np.concatenate([[0], np.cumsum(np.bincount(g, minlength=first.size))]).astype(np.int64)
+        return rows, offsets
+
+    def evaluate(self, predicted, actual_labels, ctx=None) -> MulticlassMetrics:
+        scores = _device_matrix(ctx, predicted)
+        labels = np.ascontiguousarray(actual_labels, dtype=np.int32).reshape(-1)
+        if labels.size != scores.rows or self.names.size != scores.rows:
+            raise ValueError("names, scores and labels need one entry per view")
+        rows, offsets = self.groups()
+        out = np.zeros((self.num_classes, self.num_classes), dtype=np.float64)
+        check(scores.ctx.handle, lib().ks_grouped_confusion_matrix(scores.ctx.handle, scores.handle, rows.ctypes.data_as(C.c_void_p),
+                                                                   offsets.ctypes.data_as(C.c_void_p), offsets.size - 1,
+                                                                   labels.ctypes.data_as(C.c_void_p), self.num_classes,
+                                                                   0 if self.policy == AVERAGE else 1, out.ctypes.data_as(C.c_void_p)))
+        return MulticlassMetrics(out)

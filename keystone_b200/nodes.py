@@ -4,6 +4,9 @@ reference nodes; the bodies marshal to the C ABI (which launches the sm_90a kern
 Reference classes (K/ = src/main/scala/keystoneml/):
   CosineRandomFeatures                K/nodes/stats/CosineRandomFeatures.scala:19-60
   StandardScaler / StandardScalerModel K/nodes/stats/StandardScaler.scala:16-59
+  Windower, Cropper, RandomPatcher,   K/nodes/images/*.scala (image views, DESIGN.md section 21)
+  CenterCornerPatcher, RandomImageTransformer
+  Sampler                             K/nodes/stats/Sampling.scala
   VectorSplitter                      K/nodes/util/VectorSplitter.scala:10-36
   VectorCombiner                      K/nodes/util/VectorCombiner.scala:11-14
   ClassLabelIndicatorsFromIntLabels   K/nodes/util/ClassLabelIndicators.scala:15-29
@@ -218,9 +221,10 @@ class _ConvHandle:
 
 class _ConvolvedImages(Dataset):
     """Lazy output of Convolver [-> SymmetricRectifier [-> Pooler]] on an image batch: the chain runs as ONE fused launch per image
-    chunk when it is materialised (``ImageVectorizer`` / ``to_numpy``)."""
+    chunk when it is materialised (``ImageVectorizer`` / ``to_numpy``).  ``images`` is a device matrix of images or ``ImageViews``,
+    whose views the launch gathers chunk by chunk."""
 
-    def __init__(self, images: DeviceMatrix, conv: "Convolver", rect=None, pool=None):
+    def __init__(self, images, conv: "Convolver", rect=None, pool=None):
         self.ctx, self.images, self.conv, self.rect, self.pool = images.ctx, images, conv, rect, pool
         self.rows = images.rows
 
@@ -232,8 +236,14 @@ class _ConvolvedImages(Dataset):
         if self.pool and self.rect is None:
             raise KeystoneError(-1, "Pooler after Convolver needs the SymmetricRectifier in between (the fused kernel's epilogue)")
         h = C.c_int64(0)
-        check(self.ctx.handle, lib().ks_convolver_apply(self.ctx.handle, self.conv._h.handle, self.images.handle, stride, size,
-                                                         float(max_val), float(alpha), C.byref(h)))
+        if isinstance(self.images, ImageViews):
+            v = self.images
+            check(self.ctx.handle, lib().ks_convolver_apply_views(self.ctx.handle, self.conv._h.handle, v.source.matrix.handle, v.source.x_dim,
+                                                                   v.source.y_dim, v.views.ctypes.data_as(C.c_void_p), v.rows, stride, size,
+                                                                   float(max_val), float(alpha), C.byref(h)))
+        else:
+            check(self.ctx.handle, lib().ks_convolver_apply(self.ctx.handle, self.conv._h.handle, self.images.handle, stride, size,
+                                                             float(max_val), float(alpha), C.byref(h)))
         rows, cols = C.c_int64(0), C.c_int64(0)
         check(self.ctx.handle, lib().ks_matrix_shape(self.ctx.handle, h.value, C.byref(rows), C.byref(cols)))
         return DeviceMatrix(self.ctx, h.value, rows.value, cols.value)
@@ -265,7 +275,11 @@ class Convolver(Transformer):
         self._h = _ConvHandle(ctx, h.value)
 
     def apply(self, data):
-        ds = _as_dataset(self.ctx, data)
+        if isinstance(data, ImageViews):
+            if (data.x_dim, data.y_dim, data.channels) != (self.x_dim, self.y_dim, self.ch):
+                raise KeystoneError(-1, "Convolver: the views' size does not match the Convolver's image size")
+            return _ConvolvedImages(data, self)
+        ds = _as_dataset(self.ctx, data.matrix if isinstance(data, ImageBatch) else data)
         if not isinstance(ds, DeviceMatrix):
             ds = ds.materialize()
         return _ConvolvedImages(ds, self)
@@ -301,7 +315,7 @@ class ImageVectorizer(Transformer):
     """``Image.toArray`` (K/nodes/images/ImageVectorizer.scala:12-16): forces the fused chain; rows are the vectorised images."""
 
     def apply(self, data):
-        if isinstance(data, _ConvolvedImages):
+        if isinstance(data, (_ConvolvedImages, ImageViews)):
             return data.materialize()
         return data
 
@@ -1253,11 +1267,48 @@ class ZCAWhitenerEstimator(Estimator):
 
 
 class StandardScalerModel(Transformer):
-    """(x - mean) [/ std] as a LinearMapper-free node is out of the hot path; the fits above centre internally
-    (BlockLinearMapper.scala:224-232).  Kept for API parity: holds the statistics a fitted model reports."""
+    """``StandardScalerModel(mean, std)`` (K/nodes/stats/StandardScaler.scala:16-31): (x - mean) [/ std], computed on the device in
+    fp64 and rounded once to fp32 (``ks_standard_scaler_apply``).  ``std=None`` only centres."""
 
-    def __init__(self, mean: np.ndarray, std: Optional[np.ndarray] = None):
-        self.mean, self.std = mean, std
+    def __init__(self, mean: np.ndarray, std: Optional[np.ndarray] = None, ctx: Optional[Context] = None):
+        self.mean, self.std, self.ctx = mean, std, ctx
+
+    def apply(self, data) -> DeviceMatrix:
+        x = _device_matrix(self.ctx, data)
+        mean = np.ascontiguousarray(self.mean, dtype=np.float64).reshape(-1)
+        std = None if self.std is None else np.ascontiguousarray(self.std, dtype=np.float64).reshape(-1)
+        if mean.size != x.cols or (std is not None and std.size != x.cols):
+            raise ValueError("StandardScalerModel: mean and std need one value per column")
+        h = C.c_int64(0)
+        check(x.ctx.handle, lib().ks_standard_scaler_apply(x.ctx.handle, x.handle, mean.ctypes.data_as(C.c_void_p),
+                                                           None if std is None else std.ctypes.data_as(C.c_void_p), C.byref(h)))
+        return DeviceMatrix(x.ctx, h.value, x.rows, x.cols)
+
+
+class StandardScaler(Estimator):
+    """``new StandardScaler(normalizeStdDev, eps)`` (StandardScaler.scala:38-59): fp64 column means and, with ``normalizeStdDev``, the
+    unbiased column std (MLlib's ``MultivariateOnlineSummarizer``), 1.0 where the std is NaN, infinite or below ``eps``.  The sums run
+    in a fixed order, so a refit is bit-identical.  Collective with several ranks (data: this rank's rows)."""
+
+    def __init__(self, normalizeStdDev: bool = True, eps: float = 1e-12, ctx: Optional[Context] = None):
+        self.normalize_std, self.eps, self.ctx = bool(normalizeStdDev), float(eps), ctx
+
+    def fit(self, data) -> StandardScalerModel:
+        x = _device_matrix(self.ctx, data)
+        mean = np.empty(x.cols, dtype=np.float64)
+        std = np.empty(x.cols, dtype=np.float64)
+        check(x.ctx.handle, lib().ks_standard_scaler_fit(x.ctx.handle, x.handle, 1 if self.normalize_std else 0, self.eps,
+                                                         mean.ctypes.data_as(C.c_void_p), std.ctypes.data_as(C.c_void_p)))
+        return StandardScalerModel(mean, std if self.normalize_std else None, x.ctx)
+
+
+def stats_normalize_rows(data, alpha: float = 1.0, ctx: Optional[Context] = None) -> DeviceMatrix:
+    """``Stats.normalizeRows(mat, alpha)`` (K/utils/Stats.scala:112-123) on the device: per row, minus the mean, over
+    sqrt(sample variance + alpha), in fp64, rounded once to fp32."""
+    x = _device_matrix(ctx, data)
+    h = C.c_int64(0)
+    check(x.ctx.handle, lib().ks_matrix_stats_normalize_rows(x.ctx.handle, x.handle, float(alpha), C.byref(h)))
+    return DeviceMatrix(x.ctx, h.value, x.rows, x.cols)
 
 
 # ------------------------------------------------------------------------------------------ LCS Fisher-vector branch
@@ -1919,3 +1970,257 @@ class DaisyExtractor(Transformer):
 
     def apply(self, data):
         return _items_in_input_order(self, data, self._extract, lambda items: items.to_list(np.float32)[0])
+
+
+# ------------------------------------------------------------------------------------------------- image views and augmentation
+# Windower, Cropper, RandomPatcher, CenterCornerPatcher and RandomImageTransformer (K/nodes/images/*.scala) as tables of views of a
+# source ImageBatch, and Sampler / MatrixUtils.sampleRows (K/nodes/stats/Sampling.scala, K/utils/MatrixUtils.scala).  Only index
+# bookkeeping runs on the host; every pixel is moved by ks_image_views or by the Convolver reading the views.  DESIGN.md section 21.
+class JavaRandom:
+    """``java.util.Random(seed)``: the 48-bit linear congruential generator, ``nextInt``, ``nextInt(bound)`` and ``nextDouble``
+    exactly as the JDK defines them, so that seeded draws match the reference's."""
+
+    _MULT, _ADD, _MASK = 0x5DEECE66D, 0xB, (1 << 48) - 1
+
+    def __init__(self, seed: int):
+        self._seed = (int(seed) ^ self._MULT) & self._MASK
+
+    def _next(self, bits: int) -> int:
+        self._seed = (self._seed * self._MULT + self._ADD) & self._MASK
+        r = self._seed >> (48 - bits)
+        return r - (1 << 32) if r >= (1 << 31) else r          # (int) of the top bits
+
+    def nextInt(self, bound: Optional[int] = None) -> int:
+        if bound is None:
+            return self._next(32)
+        bound = int(bound)
+        if bound <= 0:
+            raise ValueError("bound must be positive")
+        r = self._next(31)
+        m = bound - 1
+        if bound & m == 0:                                     # a power of two
+            return (bound * r) >> 31
+        u = r
+        r = u % bound
+        while u - r + m >= (1 << 31):                          # u - r + m overflows int: reject and draw again
+            u = self._next(31)
+            r = u % bound
+        return r
+
+    def nextDouble(self) -> float:
+        return ((self._next(26) << 27) + self._next(27)) * (1.0 / (1 << 53))
+
+
+class _FlipHorizontal:
+    """``ImageUtils.flipHorizontal``: reverses every image along y (ImageUtils.scala:399-420)."""
+
+    def __repr__(self) -> str:
+        return "flip_horizontal"
+
+
+flip_horizontal = _FlipHorizontal()
+
+
+class ImageViews(ImageBatch):
+    """Views of a source ``ImageBatch``, all ``x_dim`` x ``y_dim``: ``views`` is an (n x 4) int32 table (src_row, x0, y0, flip), view v
+    being ``ImageUtils.crop(src, x0, y0, x0 + x_dim, y0 + y_dim)``, reversed along y when flip is 1.  Lazy: ``matrix`` (and
+    ``ImageVectorizer`` / ``to_numpy``) gathers the views on the device; a ``Convolver`` reads them without materialising them."""
+
+    def __init__(self, source: ImageBatch, views, x_dim: int, y_dim: int):
+        views = np.ascontiguousarray(views, dtype=np.int32).reshape(-1, 4)
+        self.ctx, self.source, self.views = source.ctx, source, views
+        self.x_dim, self.y_dim, self.channels = int(x_dim), int(y_dim), source.channels
+        self._matrix: Optional[DeviceMatrix] = None
+
+    @property
+    def rows(self) -> int:
+        return int(self.views.shape[0])
+
+    @property
+    def matrix(self) -> DeviceMatrix:
+        if self._matrix is None:
+            s = self.source
+            h = C.c_int64(0)
+            check(self.ctx.handle, lib().ks_image_views(self.ctx.handle, s.matrix.handle, s.x_dim, s.y_dim, s.channels,
+                                                        self.views.ctypes.data_as(C.c_void_p), self.rows, self.x_dim, self.y_dim,
+                                                        C.byref(h)))
+            self._matrix = DeviceMatrix(self.ctx, h.value, self.rows, self.x_dim * self.y_dim * self.channels)
+        return self._matrix
+
+    def materialize(self) -> DeviceMatrix:
+        return self.matrix
+
+    def to_numpy(self, dtype=np.float64) -> np.ndarray:
+        return self.matrix.to_numpy(dtype)
+
+    def take(self, rows) -> "ImageViews":
+        """The views at these positions of the table, in that order (nothing is gathered)."""
+        return ImageViews(self.source, self.views[np.asarray(rows, dtype=np.int64)], self.x_dim, self.y_dim)
+
+
+def _view_base(node, data):
+    """(source batch, its (n x 4) views, x_dim, y_dim): an ImageViews as it is, any other image batch as one whole view per image."""
+    if isinstance(data, ImageViews):
+        return data.source, data.views, data.x_dim, data.y_dim
+    if not isinstance(data, ImageBatch):
+        data = _image_batches(node, data)[0][0]
+    n = data.rows
+    base = np.zeros((n, 4), dtype=np.int32)
+    base[:, 0] = np.arange(n)
+    return data, base, data.x_dim, data.y_dim
+
+
+def _crop_views(node, data, local: np.ndarray, out_x: int, out_y: int) -> ImageViews:
+    """local: (m x 4) (image, x0, y0, flip) relative to the input images (image = row of the input batch); composed with the
+    input's own views so that the result is a table of views of the source batch."""
+    src, base, x_dim, y_dim = _view_base(node, data)
+    local = np.asarray(local, dtype=np.int64).reshape(-1, 4)
+    if local.size and ((local[:, 1] < 0).any() or (local[:, 1] + out_x > x_dim).any() or (local[:, 2] < 0).any()
+                       or (local[:, 2] + out_y > y_dim).any() or out_x < 1 or out_y < 1):
+        raise KeystoneError(-1, "invalid crop: the view leaves the image")
+    b = base[local[:, 0]].astype(np.int64)
+    flipped = b[:, 3] == 1
+    out = np.empty_like(local)
+    out[:, 0] = b[:, 0]
+    out[:, 1] = b[:, 1] + local[:, 1]
+    # a crop of a flipped view is the mirrored range of the source, still flipped
+    out[:, 2] = np.where(flipped, b[:, 2] + y_dim - local[:, 2] - out_y, b[:, 2] + local[:, 2])
+    out[:, 3] = b[:, 3] ^ local[:, 3]
+    return ImageViews(src, out, out_x, out_y)
+
+
+class Windower(Transformer):
+    """``new Windower(stride, windowSize)`` (K/nodes/images/Windower.scala): every windowSize x windowSize window at x, y = 0, stride,
+    ... <= dim - windowSize, x outer and y inner, per image in order.  Returns ``ImageViews``."""
+
+    def __init__(self, stride: int, windowSize: int, ctx: Optional[Context] = None):
+        self.stride, self.window, self.ctx = int(stride), int(windowSize), ctx
+        if self.stride < 1 or self.window < 1:
+            raise ValueError("stride and windowSize must be >= 1")
+
+    def views(self, n_images: int, x_dim: int, y_dim: int) -> np.ndarray:
+        xs = np.arange(0, x_dim - self.window + 1, self.stride)
+        ys = np.arange(0, y_dim - self.window + 1, self.stride)
+        per = np.stack([np.repeat(xs, ys.size), np.tile(ys, xs.size)], 1)
+        out = np.zeros((n_images * per.shape[0], 4), dtype=np.int64)
+        out[:, 0] = np.repeat(np.arange(n_images), per.shape[0])
+        out[:, 1:3] = np.tile(per, (n_images, 1))
+        return out
+
+    def apply(self, data) -> ImageViews:
+        _, base, x_dim, y_dim = _view_base(self, data)
+        return _crop_views(self, data, self.views(base.shape[0], x_dim, y_dim), self.window, self.window)
+
+
+class Cropper(Transformer):
+    """``Cropper(startX, startY, endX, endY)`` (K/nodes/images/Cropper.scala): ``ImageUtils.crop`` of every image."""
+
+    def __init__(self, startX: int, startY: int, endX: int, endY: int, ctx: Optional[Context] = None):
+        self.sx, self.sy, self.ex, self.ey, self.ctx = int(startX), int(startY), int(endX), int(endY), ctx
+
+    def apply(self, data) -> ImageViews:
+        _, base, _, _ = _view_base(self, data)
+        n = base.shape[0]
+        local = np.stack([np.arange(n), np.full(n, self.sx), np.full(n, self.sy), np.zeros(n, dtype=np.int64)], 1)
+        return _crop_views(self, data, local, self.ex - self.sx, self.ey - self.sy)
+
+
+class RandomPatcher(Transformer):
+    """``RandomPatcher(numPatches, patchSizeX, patchSizeY, seed)`` (K/nodes/images/RandomPatcher.scala): per image, numPatches crops
+    with ``startX = rnd.nextInt(xDim - patchSizeX + 1)`` and then ``startY = rnd.nextInt(yDim - patchSizeY + 1)``, ``rnd`` a
+    ``java.util.Random(seed)``.  Spark hands every partition a fresh copy of the node, so the stream restarts from the seed on each
+    partition; here it restarts on every call, a call being one rank's shard.  Returns ``ImageViews``."""
+
+    def __init__(self, numPatches: int, patchSizeX: int, patchSizeY: int, seed: int = 12334, ctx: Optional[Context] = None):
+        self.n, self.px, self.py, self.seed, self.ctx = int(numPatches), int(patchSizeX), int(patchSizeY), int(seed), ctx
+
+    def views(self, n_images: int, x_dim: int, y_dim: int) -> np.ndarray:
+        if self.px > x_dim or self.py > y_dim or self.px < 1 or self.py < 1:
+            raise KeystoneError(-1, "RandomPatcher: the patch must fit in the image")
+        rnd = JavaRandom(self.seed)
+        out = np.zeros((n_images * self.n, 4), dtype=np.int64)
+        for v in range(n_images * self.n):
+            out[v, 0] = v // self.n
+            out[v, 1] = rnd.nextInt(x_dim - self.px + 1)
+            out[v, 2] = rnd.nextInt(y_dim - self.py + 1)
+        return out
+
+    def apply(self, data) -> ImageViews:
+        _, base, x_dim, y_dim = _view_base(self, data)
+        return _crop_views(self, data, self.views(base.shape[0], x_dim, y_dim), self.px, self.py)
+
+
+class CenterCornerPatcher(Transformer):
+    """``CenterCornerPatcher(patchSizeX, patchSizeY, horizontalFlips)`` (K/nodes/images/CenterCornerPatcher.scala): per image the
+    crops at the four corners and the centre, in the reference's order, each followed by its flip when ``horizontalFlips``."""
+
+    def __init__(self, patchSizeX: int, patchSizeY: int, horizontalFlips: bool, ctx: Optional[Context] = None):
+        self.px, self.py, self.flips, self.ctx = int(patchSizeX), int(patchSizeY), bool(horizontalFlips), ctx
+
+    def views(self, n_images: int, x_dim: int, y_dim: int) -> np.ndarray:
+        bx, by = x_dim - self.px, y_dim - self.py
+        starts = [(0, 0), (bx, 0), (0, by), (bx, by), (bx // 2, by // 2)]
+        per = [(x, y, f) for x, y in starts for f in ((0, 1) if self.flips else (0,))]
+        out = np.zeros((n_images * len(per), 4), dtype=np.int64)
+        out[:, 0] = np.repeat(np.arange(n_images), len(per))
+        out[:, 1:] = np.tile(np.asarray(per, dtype=np.int64), (n_images, 1))
+        return out
+
+    def apply(self, data) -> ImageViews:
+        _, base, x_dim, y_dim = _view_base(self, data)
+        return _crop_views(self, data, self.views(base.shape[0], x_dim, y_dim), self.px, self.py)
+
+
+class RandomImageTransformer(Transformer):
+    """``RandomImageTransformer(chance, transform, seed)`` (K/nodes/images/RandomImageTransformer.scala): per image in order, the
+    transform applies when ``rnd.nextDouble() < chance``, ``rnd`` a ``java.util.Random(seed)`` restarted on every call (one rank's
+    shard, as RandomPatcher).  The transform must be ``flip_horizontal``, which toggles the flip of a view; there is no host path
+    for any other function.  Returns ``ImageViews``."""
+
+    def __init__(self, chance: float, transform, seed: int = 12334, ctx: Optional[Context] = None):
+        if transform is not flip_horizontal:
+            raise KeystoneError(-1, "RandomImageTransformer: only flip_horizontal runs on the device")
+        self.chance, self.transform, self.seed, self.ctx = float(chance), transform, int(seed), ctx
+
+    def flips(self, n: int) -> np.ndarray:
+        rnd = JavaRandom(self.seed)
+        return np.array([1 if rnd.nextDouble() < self.chance else 0 for _ in range(n)], dtype=np.int32)
+
+    def apply(self, data) -> ImageViews:
+        src, base, x_dim, y_dim = _view_base(self, data)
+        views = base.copy()
+        views[:, 3] ^= self.flips(views.shape[0])
+        return ImageViews(src, views, x_dim, y_dim)
+
+
+def _sample_indices(n: int, size: int, seed: int) -> np.ndarray:
+    return np.random.default_rng(seed).choice(n, min(int(size), n), replace=False).astype(np.int64)
+
+
+class Sampler(Transformer):
+    """``new Sampler(size, seed)`` (K/nodes/stats/Sampling.scala): ``takeSample(false, size, seed)``.  Spark's draw depends on the
+    partitioning and is not reproduced: the rows are ``numpy.random.default_rng(seed).choice(n, min(size, n), replace=False)``.  On
+    ``ImageViews`` the view table is subset before anything is gathered; on a device matrix the rows are gathered on the device."""
+
+    def __init__(self, size: int, seed: int = 42, ctx: Optional[Context] = None):
+        self.size, self.seed, self.ctx = int(size), int(seed), ctx
+
+    def apply(self, data):
+        if isinstance(data, ImageViews):
+            return data.take(_sample_indices(data.rows, self.size, self.seed))
+        x = _device_matrix(self.ctx, data)
+        return _gather_rows(x, _sample_indices(x.rows, self.size, self.seed))
+
+
+def sample_rows(data, num_samples: int, seed: int = 42, ctx: Optional[Context] = None) -> DeviceMatrix:
+    """``MatrixUtils.sampleRows`` (K/utils/MatrixUtils.scala:116-119): ``num_samples`` distinct rows, drawn as by ``Sampler``
+    (the reference's unseeded ``Random.shuffle`` is not reproduced) and kept in ascending order as the reference sorts them."""
+    x = _device_matrix(ctx, data)
+    return _gather_rows(x, np.sort(_sample_indices(x.rows, num_samples, seed)))
+
+
+def _gather_rows(x: DeviceMatrix, rows: np.ndarray) -> DeviceMatrix:
+    rows = np.ascontiguousarray(rows, dtype=np.int64)
+    h = C.c_int64(0)
+    check(x.ctx.handle, lib().ks_matrix_gather_rows(x.ctx.handle, x.handle, rows.ctypes.data_as(C.c_void_p), rows.size, C.byref(h)))
+    return DeviceMatrix(x.ctx, h.value, rows.size, x.cols)
