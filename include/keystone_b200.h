@@ -362,6 +362,27 @@ KS_API int32_t ks_sparse_lbfgs_fit(int64_t ctx, int64_t s, int64_t labels, int32
  * new N x k fp32 matrix.  KS_ERR_INVALID for a model with feature means, a kernel model, or n_cols != the model's d. */
 KS_API int32_t ks_model_apply_sparse(int64_t ctx, int64_t model, int64_t s, int64_t* out_predictions);
 
+/* ---- logistic regression and multinomial naive Bayes (DESIGN.md section 22) ---------------------------------------------------
+ * Both take this rank's rows from exactly one feature source -- a dense fp32 matrix handle (features_or_0) or a sparse handle
+ * (sparse_or_0), the other 0 -- and labels: n_labels class ids in [0, num_classes) on the host (n_labels = the rank's rows,
+ * num_classes >= 2).  A label outside the range on any rank (and, for naive Bayes, a negative or NaN feature value or a class with no
+ * rows over all ranks) is flagged, all-reduced and rejected on every rank with KS_ERR_INVALID.  Every sum has a fixed order: one rank
+ * fitting the same input twice gets a bit-identical model, and every rank ends with the same bits.  Both are collective and return an
+ * ordinary model handle (d x k in feature blocks of min(d, 4096) rows, no feature means). */
+/* LogisticRegressionEstimator(numClasses, regParam, numIters, convergenceTol).fit (K/nodes/learning/LogisticRegressionModel.scala,
+ * MLlib's LogisticGradient + SquaredL2Updater): minimises (1/N) sum_i [lse(0, Z_i) - Z_{i,y_i}] + reg_param / 2 |W|^2 over W
+ * (d x (k-1), Z = A W, class 0 the pivot) from W = 0 by L-BFGS (10 corrections, the stop rules of ks_lbfgs_fit) with a strong-Wolfe
+ * line search in fp64.  The model's column 0 is zero and it has no intercept, so ks_model_apply_argmax is MLlib's predict.
+ * ks_last_fit_stats_json: solver "logistic_regression", iterations, loss_history, stop_reason (also "line_search_failed"),
+ * line_search_evals (trials per line search), per-phase device ms.  num_iterations >= 1, reg_param and convergence_tol finite, >= 0. */
+KS_API int32_t ks_logistic_fit(int64_t ctx, int64_t features_or_0, int64_t sparse_or_0, const int32_t* labels, int64_t n_labels,
+                               int32_t num_classes, double reg_param, int32_t num_iterations, double convergence_tol, int64_t* out_model);
+/* NaiveBayesEstimator(numClasses, lambda).fit (K/nodes/learning/NaiveBayesModel.scala, MLlib's multinomial NaiveBayes.train):
+ * W = theta^T with theta_cj = log(S_jc + lambda) - log(sum_j S_jc + d lambda), S_jc the sum of feature j over class c, and intercept
+ * pi_c = log(n_c + lambda) - log(N + k lambda).  lambda finite and >= 0.  ks_last_fit_stats_json: solver "naive_bayes". */
+KS_API int32_t ks_naive_bayes_fit(int64_t ctx, int64_t features_or_0, int64_t sparse_or_0, const int32_t* labels, int64_t n_labels,
+                                  int32_t num_classes, double lambda, int64_t* out_model);
+
 /* ---- covariance-based transforms (DESIGN.md section 15) -------------------------------------
  * Every product of these fits runs in fp64 on the DMMA tensor core; they take no precision mode.  The fitted objects are ordinary
  * model handles (apply, save / load, host views): apply runs in the context's precision like every model.  x: this rank's rows

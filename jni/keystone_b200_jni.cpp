@@ -189,6 +189,26 @@ JFN(jlong, modelApplySparse)(JNIEnv* env, jobject, jlong ctx, jlong model, jlong
   int64_t h = 0;
   return ok(env, ctx, ks_model_apply_sparse(ctx, model, s, &h)) ? h : 0;
 }
+// logistic regression / naive Bayes: exactly one of features and sparse is a handle; classes holds the partition's class ids
+JFN(jlong, logisticFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong sparse, jintArray classes, jint numClasses,
+                        jdouble regParam, jint numIters, jdouble convergenceTol) {
+  int64_t h = 0;
+  const jsize n = classes ? env->GetArrayLength(classes) : 0;
+  jint* p = n ? env->GetIntArrayElements(classes, nullptr) : nullptr;
+  const int32_t rc = ks_logistic_fit(ctx, features, sparse, reinterpret_cast<const int32_t*>(p), n, numClasses, regParam, numIters,
+                                     convergenceTol, &h);
+  if (p) env->ReleaseIntArrayElements(classes, p, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, naiveBayesFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong sparse, jintArray classes, jint numClasses,
+                          jdouble lambda) {
+  int64_t h = 0;
+  const jsize n = classes ? env->GetArrayLength(classes) : 0;
+  jint* p = n ? env->GetIntArrayElements(classes, nullptr) : nullptr;
+  const int32_t rc = ks_naive_bayes_fit(ctx, features, sparse, reinterpret_cast<const int32_t*>(p), n, numClasses, lambda, &h);
+  if (p) env->ReleaseIntArrayElements(classes, p, JNI_ABORT);
+  return ok(env, ctx, rc) ? h : 0;
+}
 JFN(jlong, linearMapFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong labels, jboolean hasLambda, jdouble lambda) {
   int64_t h = 0;
   return ok(env, ctx, ks_linear_map_fit(ctx, features, labels, hasLambda ? 1 : 0, lambda, &h)) ? h : 0;

@@ -119,6 +119,8 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_sparse_densify", i64, i64, p_i64)
     sig("ks_sparse_lbfgs_fit", i64, i64, i64, i32, i32, f64, i32, f64, p_i64)
     sig("ks_model_apply_sparse", i64, i64, i64, p_i64)
+    sig("ks_logistic_fit", i64, i64, i64, C.c_void_p, i64, i32, f64, i32, f64, p_i64)
+    sig("ks_naive_bayes_fit", i64, i64, i64, C.c_void_p, i64, i32, f64, p_i64)
     sig("ks_pca_fit", i64, i64, i32, p_i64)
     sig("ks_zca_fit", i64, i64, f64, p_i64)
     sig("ks_approx_range", i64, i64, C.c_void_p, i32, i32, p_i64)

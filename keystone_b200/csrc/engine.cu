@@ -2062,6 +2062,22 @@ KS_API int32_t ks_model_apply_sparse(int64_t ctx, int64_t model, int64_t s, int6
   });
 }
 
+// ---------------------------------------------------------------- logistic regression, naive Bayes (logistic.cu)
+KS_API int32_t ks_logistic_fit(int64_t ctx, int64_t features_or_0, int64_t sparse_or_0, const int32_t* labels, int64_t n_labels,
+                               int32_t num_classes, double reg_param, int32_t num_iterations, double convergence_tol, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    *out_model = fit_logistic(c, features_or_0, sparse_or_0, labels, n_labels, num_classes, reg_param, num_iterations, convergence_tol);
+  });
+}
+KS_API int32_t ks_naive_bayes_fit(int64_t ctx, int64_t features_or_0, int64_t sparse_or_0, const int32_t* labels, int64_t n_labels,
+                                  int32_t num_classes, double lambda, int64_t* out_model) {
+  return guard(ctx, [&](Ctx& c) {
+    if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
+    *out_model = fit_naive_bayes(c, features_or_0, sparse_or_0, labels, n_labels, num_classes, lambda);
+  });
+}
+
 KS_API int32_t ks_linear_map_fit(int64_t ctx, int64_t features, int64_t labels, int32_t has_lambda, double lambda, int64_t* out_model) {
   return guard(ctx, [&](Ctx& c) {
     if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};

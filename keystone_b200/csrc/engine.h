@@ -405,6 +405,20 @@ int64_t approx_range(Ctx& c, Matrix& X, const double* omega_colmajor, int l, int
 int64_t fit_approx_pca(Ctx& c, Matrix& X, const double* omega_colmajor, int dims, int q, int p);
 // out (m x n, row-major fp64, host) = (A - 1 s^T)^T (B - 1 t^T); B null: symmetric mode.  Not collective.
 void debug_gram_f64(Ctx& c, Matrix& A, Matrix* B, const double* shift_a, const double* shift_b, double* out, int64_t ld_out);
+// The fp64 DMMA products of pca.cu, on c.st.  An operand is row-major with exactly one of f32 (fp32 device matrix) / f64 set; its
+// column shift (may be null) is subtracted in fp64 as it is loaded.
+struct GramOperand {
+  const float* f32 = nullptr;
+  const double* f64 = nullptr;
+  int64_t ld = 0;
+  int cols = 0;
+  const double* shift = nullptr;
+};
+// out (a.cols x b.cols, row-major, ld ldo) = (A - 1 s^T)^T (B - 1 t^T) over `rows` rows; b null: symmetric mode (B = A).  Split-K over
+// rows with the partials summed in split order: deterministic.  rows = 0 writes zeros.  flops (may be null) += the product's flops.
+void gram_f64(Ctx& c, const GramOperand& a, const GramOperand* b, int64_t rows, double* out, int64_t ldo, double* flops = nullptr);
+// Y (rows x l, row-major, ld ldy) = A B for A = a (rows x a.cols, no shift) and a row-major fp64 B (a.cols x l, ld ldb)
+void skinny_f64(Ctx& c, const GramOperand& a, int64_t rows, const double* B, int64_t ldb, int l, double* Y, int64_t ldy);
 
 // LCS descriptors, GMM posteriors, Fisher vectors and row normalisation (fisher.cu); none is collective
 std::unique_ptr<Matrix> lcs_extract(Ctx& c, Matrix& images, int x_dim, int y_dim, int channels, int stride, int stride_start,
@@ -503,5 +517,10 @@ std::unique_ptr<Matrix> sparse_model_apply(Ctx& c, Model& m, const SparseMat& s)
 // SparseLBFGSwithL2 (lbfgs.cu); collective
 int64_t fit_sparse_lbfgs(Ctx& c, const SparseMat& s, Matrix& Y, bool fit_intercept, int num_corrections, double convergence_tol,
                          int num_iterations, double reg_param);
+// LogisticRegressionEstimator and NaiveBayesEstimator (logistic.cu); collective.  Exactly one of features / sparse is a handle, the
+// other 0; labels: the rank's n_labels class ids (host).
+int64_t fit_logistic(Ctx& c, int64_t features, int64_t sparse, const int32_t* labels, int64_t n_labels, int num_classes, double reg_param,
+                     int num_iterations, double convergence_tol);
+int64_t fit_naive_bayes(Ctx& c, int64_t features, int64_t sparse, const int32_t* labels, int64_t n_labels, int num_classes, double lambda);
 
 }  // namespace ks

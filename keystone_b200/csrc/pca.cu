@@ -292,20 +292,12 @@ __global__ void lower_only_kernel(double* __restrict__ L, int l, const int* __re
 __global__ void info_to_flag_kernel(const int* __restrict__ info, double* __restrict__ flag) { *flag = static_cast<double>(*info); }
 
 // ------------------------------------------------------------------------------------ launchers
-// DMMA Gram.  a32 / a64: exactly one is set (fp32 device matrix or fp64 buffer); b null: symmetric mode (B = A, sb ignored).
-struct GramOperand {
-  const float* f32 = nullptr;
-  const double* f64 = nullptr;
-  int64_t ld = 0;
-  int cols = 0;
-  const double* shift = nullptr;
-};
 template <class TA, class TB>
 static void gram_launch(dim3 grid, const TA* A, const GramOperand& a, const TB* B, const GramOperand& b, int64_t rows, int64_t rps, int sym,
                         double* out, int64_t ldo, double* part, cudaStream_t st) {
   gram_f64_kernel<TA, TB><<<grid, kPThreads, 0, st>>>(A, a.ld, a.shift, a.cols, B, b.ld, b.shift, b.cols, rows, rps, sym, out, ldo, part);
 }
-static void gram_f64(Ctx& c, const GramOperand& a, const GramOperand* b, int64_t rows, double* out, int64_t ldo, double* flops = nullptr) {
+void gram_f64(Ctx& c, const GramOperand& a, const GramOperand* b, int64_t rows, double* out, int64_t ldo, double* flops) {
   const bool sym = b == nullptr;
   const GramOperand& bb = sym ? a : *b;
   const int m = a.cols, n = bb.cols;
@@ -339,7 +331,7 @@ static void gram_f64(Ctx& c, const GramOperand& a, const GramOperand* b, int64_t
   }
   if (flops) *flops += 2.0 * static_cast<double>(rows) * m * n * (sym ? 0.5 : 1.0);
 }
-static void skinny_f64(Ctx& c, const GramOperand& a, int64_t rows, const double* B, int64_t ldb, int l, double* Y, int64_t ldy) {
+void skinny_f64(Ctx& c, const GramOperand& a, int64_t rows, const double* B, int64_t ldb, int l, double* Y, int64_t ldy) {
   if (rows == 0 || l == 0) return;
   const int64_t nct = (l + kPT - 1) / kPT, nrt = (rows + kPT - 1) / kPT;
   if (nct * nrt > 0x7fffffffLL) throw KsError{KS_ERR_INVALID, "too many rows for the skinny product"};

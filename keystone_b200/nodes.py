@@ -21,6 +21,8 @@ Reference classes (K/ = src/main/scala/keystoneml/):
   LeastSquaresSparseGradient          K/nodes/learning/Gradient.scala
   SparseLinearMapper                  K/nodes/learning/SparseLinearMapper.scala
   Densify                             K/nodes/util/Densify.scala
+  LogisticRegressionEstimator / Model K/nodes/learning/LogisticRegressionModel.scala
+  NaiveBayesEstimator / Model         K/nodes/learning/NaiveBayesModel.scala
 
 Batches are ``DeviceMatrix`` / ``LazyFeatures`` (this rank's rows); 2-D numpy arrays are uploaded on
 the fly when a ``Context`` was given to the node.  No node computes on the host.
@@ -795,6 +797,180 @@ class SparseLBFGSwithL2(LabelEstimator, WeightedNode):
         network = 2.0 * d * k * math.log(num_machines) / math.log(2.0)
         return self.num_iterations * (self.sparse_overhead * max(cpu_weight * flops, mem_weight * bytes_scanned)
                                       + network_weight * network)
+
+
+# ------------------------------------------------------------------------------------------ classifiers (DESIGN.md section 22)
+def _classifier_input(ctx: Optional[Context], data):
+    """A fit's feature source: (features handle or 0, sparse handle or 0, context, rows, columns).  Lazy sources are refused."""
+    if isinstance(data, SparseMatrix):
+        return 0, data.handle, data.ctx, data.rows, data.cols
+    if isinstance(data, Dataset) and not isinstance(data, DeviceMatrix):
+        raise KeystoneError(-1, f"{type(data).__name__} is not accepted here: pass a DeviceMatrix or a SparseMatrix")
+    if not isinstance(data, Dataset) and hasattr(data, "indptr"):
+        data = _as_sparse(ctx, data)
+        return 0, data.handle, data.ctx, data.rows, data.cols
+    dm = _as_dataset(ctx, data)
+    return dm.handle, 0, dm.ctx, dm.rows, dm.cols
+
+
+def _class_labels(labels, rows: int) -> np.ndarray:
+    y = np.asarray(labels)
+    if y.ndim != 1 or y.shape[0] != rows:
+        raise KeystoneError(-1, f"labels must be a 1-D array of {rows} class ids")
+    if y.size and not np.all(y == np.round(y)):
+        raise KeystoneError(-1, "labels must be integer class ids")
+    return np.ascontiguousarray(y, dtype=np.int32)
+
+
+def _first_max(scores: np.ndarray) -> np.ndarray:
+    return np.argmax(scores, axis=-1).astype(np.float64)
+
+
+class LogisticRegressionModel(BlockLinearMapper):
+    """LogisticRegressionModel (K/nodes/learning/LogisticRegressionModel.scala): MLlib's model without an intercept, stored as an
+    ordinary d x k model whose column 0 is zero (the pivot class).  ``apply`` returns float64 class ids, MLlib's ``predict``: the
+    first maximum of [0, x . w_1, ..., x . w_(k-1)].  ``weights`` is MLlib's flattened (k-1) * d vector, class-major."""
+
+    intercept = 0.0
+
+    def __init__(self, ctx: Context, handle: int):
+        super().__init__(ctx, handle)
+
+    @property
+    def num_classes(self) -> int:
+        return self.k
+
+    @property
+    def num_features(self) -> int:
+        return int(sum(w.shape[0] for w in self.xs))
+
+    @property
+    def weights(self) -> np.ndarray:
+        W = np.concatenate(self.xs, 0)
+        return np.ascontiguousarray(W[:, 1:].T).ravel()
+
+    def apply(self, data):
+        if isinstance(data, np.ndarray) and data.ndim == 1:
+            return float(self.apply(data[None, :])[0])
+        if isinstance(data, SparseMatrix) or (not isinstance(data, Dataset) and hasattr(data, "indptr")):
+            sm = _as_sparse(self.ctx, data)
+            h = C.c_int64(0)
+            check(self.ctx.handle, lib().ks_model_apply_sparse(self.ctx.handle, self.handle, sm.handle, C.byref(h)))
+            return _first_max(DeviceMatrix(self.ctx, h.value, sm.rows, self.k).to_numpy(np.float32))
+        return self.apply_argmax(data).astype(np.float64)
+
+
+class LogisticRegressionEstimator(LabelEstimator):
+    """``LogisticRegressionEstimator(numClasses, regParam, numIters, convergenceTol, numFeatures)``
+    (K/nodes/learning/LogisticRegressionModel.scala) on the device, fp64 throughout: MLlib's LogisticGradient with SquaredL2Updater,
+    no intercept, no feature scaling, by L-BFGS (10 corrections) with a strong-Wolfe line search modelled on Breeze's
+    (DESIGN.md section 22).  ``convergence_tol`` is honoured (the reference does not pass it on).  ``fit(data, labels)`` takes a
+    ``DeviceMatrix`` or ``SparseMatrix`` (this rank's rows) and the rank's class ids; collective with several ranks.
+    ``loss_history``, ``iterations``, ``stop_reason``, ``line_search_evals`` and ``stats`` are set after a fit."""
+
+    def __init__(self, num_classes: int, reg_param: float = 0.0, num_iters: int = 100, convergence_tol: float = 1e-4,
+                 num_features: int = -1, ctx: Optional[Context] = None):
+        if int(num_classes) < 2:
+            raise ValueError("num_classes must be >= 2")
+        if int(num_iters) < 1:
+            raise ValueError("num_iters must be >= 1")
+        reg_param, convergence_tol = float(reg_param), float(convergence_tol)
+        if not (reg_param >= 0.0 and math.isfinite(reg_param)):
+            raise ValueError("reg_param must be finite and >= 0")
+        if not (convergence_tol >= 0.0 and math.isfinite(convergence_tol)):
+            raise ValueError("convergence_tol must be finite and >= 0")
+        self.num_classes, self.reg_param, self.num_iters = int(num_classes), reg_param, int(num_iters)
+        self.convergence_tol, self.num_features, self.ctx = convergence_tol, int(num_features), ctx
+        self.loss_history: Optional[List[float]] = None
+        self.iterations: Optional[int] = None
+        self.stop_reason: Optional[str] = None
+        self.line_search_evals: Optional[List[int]] = None
+        self.stats: Optional[dict] = None
+
+    def fit(self, data, labels) -> LogisticRegressionModel:
+        f, s, ctx, rows, cols = _classifier_input(self.ctx, data)
+        if self.num_features not in (-1, cols):
+            raise KeystoneError(-1, f"num_features is {self.num_features} but the data has {cols} columns")
+        y = _class_labels(labels, rows)
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_logistic_fit(ctx.handle, f, s, y.ctypes.data_as(C.c_void_p), rows, self.num_classes, self.reg_param,
+                                                 self.num_iters, self.convergence_tol, C.byref(h)))
+        model = LogisticRegressionModel(ctx, h.value)
+        self.stats = ctx.last_fit_stats()
+        self.loss_history = [float(v) for v in self.stats["loss_history"]]
+        self.iterations, self.stop_reason = int(self.stats["iterations"]), self.stats["stop_reason"]
+        self.line_search_evals = [int(v) for v in self.stats["line_search_evals"]]
+        return model
+
+
+class NaiveBayesModel(BlockLinearMapper):
+    """NaiveBayesModel(labels, pi, theta) (K/nodes/learning/NaiveBayesModel.scala): ``apply`` gives the log-posteriors
+    x theta^T + pi (follow it with ``MaxClassifier``).  Stored as an ordinary model, W = theta^T (d x k) in feature blocks of
+    min(d, 4096) rows and intercept pi.  ``NaiveBayesModel(labels, pi, theta, ctx=ctx)`` builds it from host arrays;
+    ``NaiveBayesModel(ctx, handle)`` wraps a fitted or loaded model (labels 0 .. k-1)."""
+
+    def __init__(self, labels, pi=None, theta=None, ctx: Optional[Context] = None):
+        if isinstance(labels, Context):   # (ctx, handle)
+            super().__init__(labels, int(pi))
+            self.labels = np.arange(self.k)
+            return
+        if ctx is None:
+            raise KeystoneError(-1, "NaiveBayesModel from host arrays needs a Context (pass ctx=)")
+        pi = np.ascontiguousarray(pi, dtype=np.float64)
+        theta = np.asarray(theta, dtype=np.float64)
+        if theta.ndim != 2 or pi.shape != (theta.shape[0],) or theta.shape[1] < 1 or len(labels) != theta.shape[0]:
+            raise ValueError("theta must be k x d, with k values in pi and in labels")
+        W = np.asfortranarray(theta.T)
+        bs = min(W.shape[0], 4096)
+        blocks = [np.asfortranarray(W[i:i + bs]) for i in range(0, W.shape[0], bs)]
+        ptrs = (C.POINTER(C.c_double) * len(blocks))(*[w.ctypes.data_as(C.POINTER(C.c_double)) for w in blocks])
+        rows = (C.c_int64 * len(blocks))(*[w.shape[0] for w in blocks])
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_model_from_host(ctx.handle, ptrs, rows, len(blocks), W.shape[1], pi.ctypes.data_as(C.c_void_p), None,
+                                                    bs, C.byref(h)))
+        super().__init__(ctx, h.value)
+        self.labels = np.asarray(labels)
+
+    @property
+    def pi(self) -> np.ndarray:
+        return np.array(self.b_opt)
+
+    @property
+    def theta(self) -> np.ndarray:
+        return np.ascontiguousarray(np.concatenate(self.xs, 0).T)
+
+    def apply(self, data):
+        if isinstance(data, SparseMatrix) or (not isinstance(data, Dataset) and hasattr(data, "indptr")):
+            sm = _as_sparse(self.ctx, data)
+            h = C.c_int64(0)
+            check(self.ctx.handle, lib().ks_model_apply_sparse(self.ctx.handle, self.handle, sm.handle, C.byref(h)))
+            return DeviceMatrix(self.ctx, h.value, sm.rows, self.k)
+        return super().apply(data)
+
+
+class NaiveBayesEstimator(LabelEstimator):
+    """``NaiveBayesEstimator(numClasses, lambda)`` (K/nodes/learning/NaiveBayesModel.scala), MLlib's multinomial NaiveBayes.train on
+    the device: pi_c = log(n_c + lam) - log(N + k lam), theta_cj = log(S_cj + lam) - log(sum_j S_cj + d lam) with S_cj the sum of
+    feature j over class c.  Negative or NaN feature values, labels outside [0, num_classes) and classes with no rows are rejected
+    (on every rank).  ``fit(data, labels)`` as for ``LogisticRegressionEstimator``; collective with several ranks."""
+
+    def __init__(self, num_classes: int, lam: float = 1.0, ctx: Optional[Context] = None):
+        if int(num_classes) < 2:
+            raise ValueError("num_classes must be >= 2")
+        lam = float(lam)
+        if not (lam >= 0.0 and math.isfinite(lam)):
+            raise ValueError("lam must be finite and >= 0")
+        self.num_classes, self.lam, self.ctx = int(num_classes), lam, ctx
+        self.stats: Optional[dict] = None
+
+    def fit(self, data, labels) -> NaiveBayesModel:
+        f, s, ctx, rows, _ = _classifier_input(self.ctx, data)
+        y = _class_labels(labels, rows)
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_naive_bayes_fit(ctx.handle, f, s, y.ctypes.data_as(C.c_void_p), rows, self.num_classes, self.lam,
+                                                    C.byref(h)))
+        self.stats = ctx.last_fit_stats()
+        return NaiveBayesModel(ctx, h.value)
 
 
 class LeastSquaresEstimator(LabelEstimator, WeightedNode):

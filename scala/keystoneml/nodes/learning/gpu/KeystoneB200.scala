@@ -42,6 +42,10 @@ class KeystoneB200 extends Serializable {
   @native def sparseLbfgsFit(ctx: Long, s: Long, labels: Long, fitIntercept: Boolean, numCorrections: Int, convergenceTol: Double,
       numIterations: Int, regParam: Double): Long
   @native def modelApplySparse(ctx: Long, model: Long, s: Long): Long
+  /** LogisticRegressionEstimator / NaiveBayesEstimator (collective): exactly one of features and sparse is a handle, the other 0. */
+  @native def logisticFit(ctx: Long, features: Long, sparse: Long, classes: Array[Int], numClasses: Int, regParam: Double, numIters: Int,
+      convergenceTol: Double): Long
+  @native def naiveBayesFit(ctx: Long, features: Long, sparse: Long, classes: Array[Int], numClasses: Int, lambda: Double): Long
   /** PCA / ZCA / approximate PCA (collective, fp64 on the device); omega is the d x l test matrix, DenseMatrix.data. */
   @native def pcaFit(ctx: Long, x: Long, dims: Int): Long
   @native def zcaFit(ctx: Long, x: Long, eps: Double): Long
