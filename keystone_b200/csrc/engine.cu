@@ -592,22 +592,51 @@ void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* s
   c.launches += 1;
 }
 
-const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, int* num_tiles) {
-  std::vector<int> key = {b, kcols, with_g ? 1 : 0, with_c ? 1 : 0};
+// Pairs of tiles for the split Gram's CTA pairs (see GramTile), every tile exactly once: the tiles j0(i), j0(i) + 1, ... of row
+// i pair along the row and share A_i; a row of odd length leaves its last tile (i, nb - 1) over, and those pair across rows and
+// share B_{nb - 1}; the last one of an odd number of them runs beside an idle partner.  upper: row i starts at j0 = i (the G
+// triangle), else at 0 (C).
+static void pair_tiles(std::vector<GramTile>& t, int mb, int nb, int which, bool upper) {
+  std::vector<GramTile> left;
+  for (int i = 0; i < mb; ++i) {
+    int j = upper ? i : 0;
+    for (; j + 1 < nb; j += 2) {
+      t.push_back(GramTile{i, j, which, 0});
+      t.push_back(GramTile{i, j + 1, which, 0});
+    }
+    if (j < nb) left.push_back(GramTile{i, j, which, GRAM_SHARE_B});
+  }
+  for (size_t q = 0; q + 1 < left.size(); q += 2) {
+    t.push_back(left[q]);
+    t.push_back(left[q + 1]);
+  }
+  if (left.size() % 2) {
+    const GramTile lone = left.back();
+    t.push_back(lone);
+    t.push_back(GramTile{lone.m_blk, lone.n_blk, which, GRAM_SHARE_B | GRAM_IDLE});
+  }
+}
+
+const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, bool split, int* num_tiles) {
+  std::vector<int> key = {b, kcols, with_g ? 1 : 0, with_c ? 1 : 0, split ? 1 : 0};
   auto it = c.tile_cache.find(key);
   std::vector<GramTile> t;
   const int tm = 128, tn = 128;
   const int mb = (b + tm - 1) / tm;
   if (with_g) {
     const int nbk = (b + tn - 1) / tn;
-    for (int i = 0; i < mb; ++i)
-      for (int j = 0; j < nbk; ++j)
-        if ((j + 1) * tn - 1 >= i * tm) t.push_back(GramTile{i, j, 0, 0});  // tile touches the upper triangle
+    if (split) pair_tiles(t, mb, nbk, 0, true);
+    else
+      for (int i = 0; i < mb; ++i)
+        for (int j = 0; j < nbk; ++j)
+          if ((j + 1) * tn - 1 >= i * tm) t.push_back(GramTile{i, j, 0, 0});  // tile touches the upper triangle
   }
   if (with_c) {
     const int nck = (kcols + tn - 1) / tn;
-    for (int i = 0; i < mb; ++i)
-      for (int j = 0; j < nck; ++j) t.push_back(GramTile{i, j, 1, 0});
+    if (split) pair_tiles(t, mb, nck, 1, false);
+    else
+      for (int i = 0; i < mb; ++i)
+        for (int j = 0; j < nck; ++j) t.push_back(GramTile{i, j, 1, 0});
   }
   *num_tiles = static_cast<int>(t.size());
   if (it != c.tile_cache.end()) return it->second->as<GramTile>();
@@ -631,7 +660,7 @@ void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int 
   int nt = 0;
   g.f16 = f16 ? 1 : 0;
   g.split = split ? 1 : 0;
-  g.tiles = gram_tiles(c, b, kcols, with_g, with_c, &nt);
+  g.tiles = gram_tiles(c, b, kcols, with_g, with_c, split, &nt);
   g.num_tiles = nt;
   const int stage_rows = split ? 32 : f16 ? 64 : kGramStageRows;
   if (f16) {  // MN-major fp16 operands: 64-column (128 B) x 64-row boxes (pairs: 32-row), plain 128 B swizzle

@@ -362,7 +362,8 @@ void produce_slab(Ctx& c, FeatSrc& src, int64_t c0, int64_t cols, const float* s
                   bool out16 = false, bool x2 = false,  // x2: unrounded slab from the K-concatenated split operands: fp32, or
                   void* slab_lo = nullptr,              // (slab_lo given) the fp16 pair hi -> slab, lo -> slab_lo written by the epilogue
                   double* colsumsq = nullptr);          // fp16 pair with colsum only (fp64[cols], zeroed): += sum of (hi + lo)^2
-const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, int* num_tiles);
+// split: the CTA-pair list of the split Gram (two entries per pair, see GramTile)
+const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, bool split, int* num_tiles);
 // f16: slab and R are fp16 matrices (leading dimensions in elements); G / C stay fp32
 void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, const void* R, int64_t ldr, int kcols,
                        float* G, int ldg, float* C, int ldc, bool with_g, bool with_c, cudaStream_t st = nullptr,

@@ -11,18 +11,22 @@ static constexpr int kPadCols = 32;        // every device matrix has ld % 32 ==
 
 enum { EPI_COS = 0, EPI_UPDATE = 1, EPI_APPLY = 2, EPI_POOL = 3, EPI_RBF = 4 };
 
+// Split Gram: its CTAs run in pairs (clusters of two) whose tiles share one operand panel, and the list holds two entries per
+// pair in rank order.  pair = 0: the two tiles share A's panel (same m_blk); GRAM_SHARE_B: they share B's (same n_blk, same
+// which); GRAM_IDLE: the entry has no tile of its own (a lone tile's partner) and repeats its partner's tile.
+enum { GRAM_SHARE_B = 1, GRAM_IDLE = 2 };
 struct GramTile {
   int m_blk;  // 128-wide block of A's columns
   int n_blk;  // 128-wide block of B's columns
   int which;  // 0: B = tmB0 -> out0,  1: B = tmB1 -> out1
-  int pad;
+  int pair;   // split Gram only: GRAM_SHARE_B | GRAM_IDLE
 };
 struct GramLaunch {
   CUtensorMap tmA, tmB0, tmB1;   // operands: tf32 box {32, kGramStageRows}, fp16 box {64, 64} (split: {64, 32}); SWIZZLE_128B
   CUtensorMap tmOut0, tmOut1;    // outputs:  box {32, 32}, SWIZZLE_128B; dims clip the reduce-add at the matrix edge
   CUtensorMap tmAlo, tmB0lo, tmB1lo;  // split only: the lo planes of A, B0, B1 (same geometry as the hi maps)
   const GramTile* tiles;         // device
-  int num_tiles;
+  int num_tiles;                 // entries of tiles (split: two per CTA pair)
   int rows;        // contraction length (rows of A and B)
   int chunk_rows;  // split of the contraction across CTAs (multiple of the stage rows)
   int n_valid0, n_valid1;  // valid output columns per target (whole 32-column chunks beyond are skipped)

@@ -18,6 +18,7 @@
 //
 // L: column-major n x n (ld = n), lower triangle valid (cusolverDnDpotrf, CUBLAS_FILL_MODE_LOWER).  B: column-major n x k.
 // Dinv: ceil(n / 64) tiles of 64 x 64 doubles, column-major inside a tile, zero above the diagonal and beyond n.
+#include "cluster.cuh"
 #include "kernels.h"
 
 namespace ks {
@@ -152,24 +153,8 @@ chol_solve_kernel(const double* __restrict__ L, const double* __restrict__ Dinv,
 // 64 x 8 partial sums in its own shared memory, the leader CTA reads them through distributed shared memory, finishes the tile
 // (B_I - sum, product with the inverted diagonal tile) and publishes the solved rows; two cluster barriers per step.  The
 // latency of the substitution (128 dependent tile steps) thus shrinks with CL: k = 125 -> 16 clusters of 8 CTAs.
-__device__ __forceinline__ uint32_t cl_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cl_nctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cl_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ double ld_dsmem_f64(const double* local_ptr, uint32_t rank) {
-  const uint32_t la = static_cast<uint32_t>(__cvta_generic_to_shared(local_ptr));
-  uint32_t ra;
-  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(la), "r"(rank));
+  const uint32_t ra = cl_map_shared(static_cast<uint32_t>(__cvta_generic_to_shared(local_ptr)), rank);
   double v;
   asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(ra));
   return v;

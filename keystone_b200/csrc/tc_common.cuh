@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "cluster.cuh"
+
 namespace ks {
 
 // Error flag written (and the kernel trapped) when a barrier wait exceeds its budget:
@@ -53,6 +55,12 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// arrive on a barrier of another CTA of the cluster (cluster_addr from cl_map_shared).  Default semantics (release at CTA scope):
+// the arrive releases a stage whose reads (wgmma, waited for) are complete, so no memory needs ordering at cluster scope, and
+// .release.cluster would put a MEMBAR.GPU in front of every arrive
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -87,6 +95,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+// The same load multicast to the CTAs of the cluster in cta_mask: the box lands at the same shared-memory offset in each of them
+// and completes bytes on the barrier at the same offset in each.
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1,
+                                               uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], "
+      "%3;" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1)
       : "memory");
 }
 

@@ -23,6 +23,7 @@
 // tile (KmSmem).
 // SPLIT variants (parity mode, fp16 pairs; Gram and EPI_UPDATE): each stage holds the hi and lo planes of both operands and one
 // pass issues hi·hi, lo·hi and hi·lo into two accumulators, so the operands are fetched and the output is reduce-added once.
+#include <algorithm>
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -177,6 +178,7 @@ struct GramCfg {
   static constexpr int A_BYTES = NBOX * BOX_BYTES;
   static_assert(PLANES * A_BYTES == kStageBytes, "stage size");
   static_assert(!SPLIT || F16, "split operands are fp16 pairs");
+  static_assert(!SPLIT || NBOX == 2, "each CTA of a pair fetches one box of each shared plane");
 };
 
 // tf32 element (column c, row r) of one MN-major operand tile: 32-column boxes of SR rows, 128 B swizzle
@@ -204,8 +206,13 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = warp >> 2;
-  const GramTile tile = tiles[blockIdx.x % num_tiles];
-  const int chunk = blockIdx.x / num_tiles;
+  // SPLIT: clusters of two CTAs, one pair of tiles each; entry 2 p + rank of the list is this CTA's tile of pair p
+  const uint32_t rank = SPLIT ? cl_ctarank() : 0;
+  const int pairs = num_tiles / 2;
+  const GramTile tile = SPLIT ? tiles[2 * ((blockIdx.x >> 1) % pairs) + rank] : tiles[blockIdx.x % num_tiles];
+  const int chunk = SPLIT ? (blockIdx.x >> 1) / pairs : blockIdx.x / num_tiles;
+  const bool idle = SPLIT && (tile.pair & GRAM_IDLE);
+  const bool share_b = SPLIT && (tile.pair & GRAM_SHARE_B);
   const int row0 = chunk * chunk_rows;
   const int nrows = min(chunk_rows, rows - row0);
   const int ksteps = (nrows + SR - 1) / SR;
@@ -225,11 +232,12 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     tma_prefetch_desc(tmOut);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&L.full_bar[s], 1);
-      mbar_init(&L.empty_bar[s], 8);  // one arrive per consumer warp
+      mbar_init(&L.empty_bar[s], SPLIT ? 16 : 8);  // one arrive per consumer warp (SPLIT: of both CTAs of the pair)
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  if (SPLIT) cl_sync();  // the partner's barriers are initialised before anything lands in or arrives on them
+  else __syncthreads();
 
   if (wg == 0) {
     if (SPLIT) setmaxnreg_dec<40>();  // two accumulators per consumer thread
@@ -237,8 +245,8 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int ks = 0; ks < ksteps; ++ks) {
         const int s = ks % kStages;
         const uint32_t ph = (ks / kStages) & 1;
-        mbar_wait(&L.empty_bar[s], ph ^ 1);
-        mbar_arrive_expect_tx(&L.full_bar[s], kStageBytes);
+        mbar_wait(&L.empty_bar[s], ph ^ 1);  // SPLIT: released by the consumers of both CTAs (the multicast writes into both)
+        mbar_arrive_expect_tx(&L.full_bar[s], idle ? kStageBytes / 2 : kStageBytes);
         uint8_t* sA = L.stages + s * kStageBytes;
         const int r = row0 + ks * SR;
         // tiles in stage order: A, B (SPLIT: A_hi, A_lo, B_hi, B_lo)
@@ -246,11 +254,21 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int pl = 0; pl < Cfg::PLANES; ++pl) {
           const int c0 = (pl < Cfg::PLANES / 2) ? m0 : n0;
+          if (SPLIT && (pl >= Cfg::PLANES / 2) == share_b) {
+            // the shared panel: this CTA fetches box `rank` of the plane for both CTAs of the pair
+            tma_load_2d_mc(sA + pl * Cfg::A_BYTES + rank * Cfg::BOX_BYTES, maps[pl], &L.full_bar[s], c0 + Cfg::CW * rank, r, 0x3);
+            continue;
+          }
+          if (idle) continue;
 #pragma unroll
           for (int i = 0; i < Cfg::NBOX; ++i)
             tma_load_2d(sA + pl * Cfg::A_BYTES + i * Cfg::BOX_BYTES, maps[pl], &L.full_bar[s], c0 + Cfg::CW * i, r);
         }
       }
+    }
+    if (SPLIT) {
+      __syncwarp();
+      cl_sync();  // neither CTA exits while the other may still write into its stages or arrive on its barriers
     }
     return;
   }
@@ -268,10 +286,20 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int i = 0; i < 64; ++i) acc_x[i] = 0.f;
     wgmma_fence_acc(acc);
     wgmma_fence_acc(acc_x);
+    // a stage is released to the producers of both CTAs: each of them refills part of it
+    const uint32_t peer_empty = cl_map_shared(smem_u32(L.empty_bar), rank ^ 1);
+    auto release = [&](int s) {
+      mbar_arrive(&L.empty_bar[s]);
+      mbar_arrive_remote(peer_empty + 8 * s);
+    };
     int prev = -1;
     for (int ks = 0; ks < ksteps; ++ks) {
       const int s = ks % kStages;
       mbar_wait(&L.full_bar[s], (ks / kStages) & 1);
+      if (idle) {  // the partner's tile alone: hand the stage back once its half of the shared panel has landed here
+        if (lane == 0) release(s);
+        continue;
+      }
       const uint32_t st = smem_u32(L.stages + s * kStageBytes);
       const uint32_t sAhi = st + g * Cfg::BOX_BYTES, sAlo = sAhi + Cfg::A_BYTES;  // this warpgroup's 64 columns of A
       const uint32_t sBhi = st + 2 * Cfg::A_BYTES, sBlo = st + 3 * Cfg::A_BYTES;
@@ -290,7 +318,7 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_commit();
       if (prev >= 0) {
         wgmma_wait<1>();
-        if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+        if (lane == 0) release(prev);
       }
       prev = s;
     }
@@ -393,8 +421,12 @@ gram_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       bulk_commit();
     }
   };
-  epilogue_slabs(raw, g, w, lane, to_raw, chunk_fn);
+  if (!idle) epilogue_slabs(raw, g, w, lane, to_raw, chunk_fn);
   if (lane == 0) bulk_wait0();
+  if (SPLIT) {
+    __syncwarp();
+    cl_sync();  // the producers' cl_sync: all remote arrivals on and multicast writes into this CTA are done
+  }
 }
 
 // =====================================================================================
@@ -643,8 +675,16 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   const int wg = warp >> 2;
   const int m_tiles = (p.M + kTileM - 1) / kTileM;
   const int n_tiles = (p.N + kTileN - 1) / kTileN;
-  const int total_tiles = m_tiles * n_tiles;
+  // SPLIT: clusters of two CTAs walk pairs of tiles (m, 2 q) and (m, 2 q + 1), which share the slab rows A_m; rank r computes
+  // tile (m, 2 q + r), or nothing when that column tile is past the end (odd n_tiles)
+  // (in a 1D grid of (2, 1, 1) clusters the rank is blockIdx.x & 1: a special register read, which the compiler may repeat instead
+  // of keeping it live beside the two accumulators)
+  const int n_pairs = (n_tiles + 1) / 2;
+  const uint32_t rank = SPLIT ? (blockIdx.x & 1) : 0;
+  const int total_tiles = SPLIT ? m_tiles * n_pairs : m_tiles * n_tiles;
   const int ksteps = (p.K + BK - 1) / BK;
+  auto tile_m0 = [&](int t) { return (t / (SPLIT ? n_pairs : n_tiles)) * kTileM; };
+  auto tile_n0 = [&](int t) { return SPLIT ? (2 * (t % n_pairs) + static_cast<int>(rank)) * kTileN : (t % n_tiles) * kTileN; };
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -656,7 +696,7 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     tma_prefetch_desc(&tmOut);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&L.full_bar[s], 1);
-      mbar_init(&L.empty_bar[s], 8);  // one arrive per consumer warp
+      mbar_init(&L.empty_bar[s], SPLIT ? 16 : 8);  // one arrive per consumer warp (SPLIT: of both CTAs of the pair)
     }
     for (int r = 0; r < 8; ++r) mbar_init(&L.ring_bar[r], 1);
     if (ASYNC) {
@@ -665,7 +705,8 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  if (SPLIT) cl_sync();  // the partner's barriers are initialised before anything lands in or arrives on them
+  else __syncthreads();
 
   // Tile schedule.  With p.tile_counter the CTAs draw tiles from a global counter: a CTA that got its SM late (this kernel is
   // persistent and shares the GPU with the factor / solve chains' kernels) simply takes fewer tiles instead of stretching the
@@ -715,32 +756,42 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   if (wg == 0) {
     if (warp == 0 && elect_one()) {
       uint32_t it = 0, tl = 0;
-      int next = p.tile_counter ? atomicAdd(p.tile_counter, 1) : static_cast<int>(blockIdx.x);
+      // SPLIT: pairs strided statically over the clusters; both CTAs of a cluster walk the same sequence
+      int next = SPLIT ? static_cast<int>(blockIdx.x >> 1)
+                       : p.tile_counter ? atomicAdd(p.tile_counter, 1) : static_cast<int>(blockIdx.x);
       for (;; ++tl) {
         const int t = next < total_tiles ? next : -1;
         L.tile_ring[tl & 7] = t;
         mbar_arrive(&L.ring_bar[tl & 7]);
         if (t < 0) break;
-        next = p.tile_counter ? atomicAdd(p.tile_counter, 1) : t + static_cast<int>(gridDim.x);  // latency hides under this tile
-        const int m0 = (t / n_tiles) * kTileM;
-        const int n0 = (t % n_tiles) * kTileN;
+        next = SPLIT ? t + static_cast<int>(gridDim.x >> 1)
+                     : p.tile_counter ? atomicAdd(p.tile_counter, 1) : t + static_cast<int>(gridDim.x);  // latency hides under this tile
+        const int m0 = tile_m0(t);
+        const int n0 = tile_n0(t);
+        const bool idle = SPLIT && n0 >= p.N;
         for (int ks = 0; ks < ksteps; ++ks, ++it) {
           const int s = it % kStages;
           const uint32_t ph = (it / kStages) & 1;
-          mbar_wait(&L.empty_bar[s], ph ^ 1);
-          mbar_arrive_expect_tx(&L.full_bar[s], kStageBytes);
+          mbar_wait(&L.empty_bar[s], ph ^ 1);  // SPLIT: released by the consumers of both CTAs (the multicast writes into both)
+          mbar_arrive_expect_tx(&L.full_bar[s], idle ? kStageBytes / 2 : kStageBytes);
           uint8_t* sA = L.stages + s * kStageBytes;
-          if (SPLIT) {  // A_hi, A_lo, B_hi, B_lo
-            tma_load_2d(sA, &tmA, &L.full_bar[s], ks * BK, m0);
-            tma_load_2d(sA + A_BYTES, &tmAlo, &L.full_bar[s], ks * BK, m0);
-            tma_load_2d(sA + 2 * A_BYTES, &tmB, &L.full_bar[s], ks * BK, n0);
-            tma_load_2d(sA + 3 * A_BYTES, &tmBlo, &L.full_bar[s], ks * BK, n0);
+          if (SPLIT) {  // A_hi, A_lo, B_hi, B_lo; rank 0 fetches A_hi and rank 1 A_lo for both CTAs of the pair
+            if (rank == 0) tma_load_2d_mc(sA, &tmA, &L.full_bar[s], ks * BK, m0, 0x3);
+            else tma_load_2d_mc(sA + A_BYTES, &tmAlo, &L.full_bar[s], ks * BK, m0, 0x3);
+            if (!idle) {
+              tma_load_2d(sA + 2 * A_BYTES, &tmB, &L.full_bar[s], ks * BK, n0);
+              tma_load_2d(sA + 3 * A_BYTES, &tmBlo, &L.full_bar[s], ks * BK, n0);
+            }
           } else {
             tma_load_2d(sA, &tmA, &L.full_bar[s], ks * BK, m0);
             tma_load_2d(sA + A_BYTES, &tmB, &L.full_bar[s], ks * BK, n0);
           }
         }
       }
+    }
+    if (SPLIT) {
+      __syncwarp();
+      cl_sync();  // neither CTA exits while the other may still write into its stages or arrive on its barriers
     }
     return;
   }
@@ -762,8 +813,23 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       return;
     }
     if (t < 0) break;
-    const int m0 = (t / n_tiles) * kTileM;
-    const int n0 = (t % n_tiles) * kTileN;
+    const int m0 = tile_m0(t);
+    const int n0 = tile_n0(t);
+
+    // SPLIT: a stage is released to the producers of both CTAs: each of them refills part of it (the partner's barrier address
+    // is formed at the arrive: nothing more stays live beside the two accumulators)
+    auto release = [&](int s) {
+      mbar_arrive(&L.empty_bar[s]);
+      if (SPLIT) mbar_arrive_remote(cl_map_shared(smem_u32(&L.empty_bar[s]), rank ^ 1));
+    };
+    if (SPLIT && n0 >= p.N) {  // the partner's tile alone: hand each stage back once this CTA's copy of A has landed
+      for (int ks = 0; ks < ksteps; ++ks, ++it) {
+        const int s = it % kStages;
+        mbar_wait(&L.full_bar[s], (it / kStages) & 1);
+        if (lane == 0) release(s);
+      }
+      continue;
+    }
 
     float acc[64];
 #pragma unroll
@@ -794,14 +860,14 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         wgmma_commit();
         if (prev >= 0) {
           wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(&L.empty_bar[prev]);
+          if (lane == 0) release(prev);
         }
         prev = s;
       }
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       wgmma_fence_acc(acc_x);
-      if (prev >= 0 && lane == 0) mbar_arrive(&L.empty_bar[prev]);
+      if (prev >= 0 && lane == 0) release(prev);
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = __fadd_rn(acc[i], acc_x[i]);
     } else {
@@ -853,6 +919,10 @@ gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     epilogue_slabs(raw, g, w, lane, to_raw, chunk_fn);
   }
   if (lane == 0) bulk_wait0();
+  if (SPLIT) {
+    __syncwarp();
+    cl_sync();  // the producers' cl_sync: all remote arrivals on and multicast writes into this CTA are done
+  }
 }
 
 // =====================================================================================
@@ -909,6 +979,42 @@ static cudaError_t set_smem_attr_once(K kern, bool& done, int bytes = kSmemBytes
   return cudaSuccess;
 }
 
+static cudaLaunchConfig_t pair_config(unsigned grid, int smem, cudaStream_t st, cudaLaunchAttribute* attr) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = static_cast<size_t>(smem);
+  cfg.stream = st;
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+// The split kernels run as clusters of two CTAs (grid even).
+template <typename K, typename... Args>
+static cudaError_t launch_pairs(K kern, unsigned grid, int smem, cudaStream_t st, Args... args) {
+  cudaLaunchAttribute attr[1];
+  const cudaLaunchConfig_t cfg = pair_config(grid, smem, st, attr);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
+  return e != cudaSuccess ? e : cudaGetLastError();
+}
+// How many pairs of a kernel can be resident at once: a cluster's two CTAs sit in one GPC, so on a GPC with an odd number of
+// free SMs one SM stays out and the count may be below num_sms / 2.  The persistent split update takes no more, or the pairs
+// that did not fit would start only when others finish, after a whole launch's worth of tiles.
+template <typename K>
+static cudaError_t resident_pairs(K kern, int smem, int num_sms, int* pairs) {
+  cudaLaunchAttribute attr[1];
+  const cudaLaunchConfig_t cfg = pair_config(static_cast<unsigned>(std::max(2, num_sms & ~1)), smem, nullptr, attr);
+  int n = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
+  if (e != cudaSuccess) return e;
+  *pairs = std::max(1, std::min(n, num_sms / 2));
+  return cudaSuccess;
+}
+
 template <bool F16, bool SPLIT>
 static cudaError_t launch_gram_t(const GramLaunch& g, cudaStream_t st) {
   if (g.chunk_rows % GramCfg<F16, SPLIT>::SR != 0) return cudaErrorInvalidValue;
@@ -919,6 +1025,11 @@ static cudaError_t launch_gram_t(const GramLaunch& g, cudaStream_t st) {
   const int chunks = (g.rows + g.chunk_rows - 1) / g.chunk_rows;
   const unsigned grid = static_cast<unsigned>(chunks) * static_cast<unsigned>(g.num_tiles);
   if (grid == 0) return cudaSuccess;
+  if (SPLIT) {  // CTA pairs: g.tiles holds two entries per pair, so the grid is chunks x pairs x 2
+    if (g.num_tiles % 2 != 0) return cudaErrorInvalidValue;
+    return launch_pairs(kern, grid, kSmemBytes, st, g.tmA, g.tmB0, g.tmB1, g.tmOut0, g.tmOut1, g.tmAlo, g.tmB0lo, g.tmB1lo, g.tiles,
+                        g.num_tiles, g.rows, g.chunk_rows, g.n_valid0, g.n_valid1);
+  }
   kern<<<grid, kThreads, kSmemBytes, st>>>(g.tmA, g.tmB0, g.tmB1, g.tmOut0, g.tmOut1, SPLIT ? g.tmAlo : g.tmA, SPLIT ? g.tmB0lo : g.tmB0,
                                            SPLIT ? g.tmB1lo : g.tmB1, g.tiles, g.num_tiles, g.rows, g.chunk_rows, g.n_valid0, g.n_valid1);
   return cudaGetLastError();
@@ -939,6 +1050,17 @@ static cudaError_t launch_km_t(const KmLaunch& k, cudaStream_t st) {
   const int n_tiles = (k.p.N + kTileN - 1) / kTileN;
   const long long total = static_cast<long long>(m_tiles) * n_tiles;
   if (total == 0) return cudaSuccess;
+  if (SPLIT) {  // clusters of two CTAs, one pair of column tiles at a time, at most as many as fit on the GPU at once
+    if (k.p.tile_counter) return cudaErrorInvalidValue;  // the pairs are strided statically
+    static int fit = 0;
+    if (!fit) {
+      e = resident_pairs(kern, km_smem_bytes(EPI), k.num_sms, &fit);
+      if (e != cudaSuccess) return e;
+    }
+    const long long pairs = static_cast<long long>(m_tiles) * ((n_tiles + 1) / 2);
+    const unsigned grid = 2u * static_cast<unsigned>(std::min<long long>(pairs, std::min(fit, std::max(1, k.num_sms / 2))));
+    return launch_pairs(kern, grid, km_smem_bytes(EPI), st, k.tmA, k.tmB, k.tmOut, k.tmOut, k.tmAlo, k.tmBlo, k.p);
+  }
   const unsigned grid = static_cast<unsigned>(total < k.num_sms ? total : k.num_sms);
   kern<<<grid, km_threads(EPI), km_smem_bytes(EPI), st>>>(k.tmA, k.tmB, k.tmOut, OUT16 == 2 ? k.tmOut2 : k.tmOut, SPLIT ? k.tmAlo : k.tmA,
                                            SPLIT ? k.tmBlo : k.tmB, k.p);
