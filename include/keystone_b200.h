@@ -535,6 +535,28 @@ KS_API int32_t ks_debug_update(int64_t ctx, int64_t a, int64_t b, int32_t apply,
  * H_out and the right-hand side (b) into rhs_out (either may be NULL, not both).  The host buffers must stay valid until
  * that fit returns; the fit disarms the context whether or not the class and block exist. */
 KS_API int32_t ks_debug_bwls_capture(int64_t ctx, int32_t block, int32_t cls, double* H_out, double* rhs_out);
+/* Adds step (sweep, block) to the steps the next ks_blockls_fit / ks_linear_map_fit on the context copies to the host; several
+ * calls request several steps of one fit.  outs[KS_BLS_CAP_COUNT]: host buffers indexed by the KS_BLS_CAP_* constants, each
+ * NULL (not wanted) or large enough for its entry below, with b that block's width, n the context's row count, k the classes.
+ * Every entry is fp64, converted exactly from what the device holds, and copied on the stream that produced it at the point
+ * listed, so the fit launches the same kernels with and without a capture.  The buffers must stay valid until that fit
+ * returns; the fit disarms the context whether or not the steps exist.  H and DIAG exist at sweep 0 only (later sweeps reuse
+ * the cached factor): requesting them for a later sweep is KS_ERR_INVALID.  The copies block the host between collectives, so
+ * with several ranks arm the same steps on every rank. */
+#define KS_BLS_CAP_SHIFT 0     /* b: the fp32 shift m_j the slab was built with, after the shift estimate */
+#define KS_BLS_CAP_DELTA 1     /* b: delta_j = mean(slab) as launch_delta_mean wrote it (mean_j = m_j + delta_j), copied in the
+                                  solve chain with RHS, after it has waited for the factor */
+#define KS_BLS_CAP_DIAG 2      /* b: the exact fp64 diagonal of S^T S, all-reduced (parity mode only), before the system assembly */
+#define KS_BLS_CAP_H 3         /* b x b column-major: H_j = S^T S - N delta delta^T + lambda I before the Cholesky factorisation */
+#define KS_BLS_CAP_RHS 4       /* b x k column-major: S^T R - delta rsum^T - lambda W_old, before the solve */
+#define KS_BLS_CAP_DW 5        /* b x k column-major: the increment dW_j, after the solve, before it is packed for the update */
+#define KS_BLS_CAP_SLAB_HI 6   /* n x b row-major: the slab S_j (hi plane of the split operands) as the Gram kernels read it */
+#define KS_BLS_CAP_SLAB_LO 7   /* n x b row-major: its lo plane (zero in the single-operand modes) */
+#define KS_BLS_CAP_R_BEFORE 8  /* n x k row-major: the fp32 residual before this step's C = S^T R */
+#define KS_BLS_CAP_R_AFTER 9   /* n x k row-major: the fp32 residual after this step's update R -= (S - 1 delta^T) dW */
+#define KS_BLS_CAP_SCALES 10   /* 4: fp16 modes' powers of two {residual s, 1/s, increment s, 1/s} (1 otherwise), with DW */
+#define KS_BLS_CAP_COUNT 11
+KS_API int32_t ks_debug_blockls_capture(int64_t ctx, int32_t sweep, int32_t block, double* const* outs);
 
 /* X = H^-1 B for a symmetric positive definite H (column-major n x n) and B (column-major n x k): Cholesky with cuSOLVER, then
  * either the library's own multi-RHS solve kernel (use_cusolver = 0; option "custom_solve") or cusolverDnDpotrs (the default of

@@ -161,6 +161,7 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_debug_time_slab", i64, i64, p_i64, i32, i32, i32, i64, i32, p_f64, C.c_void_p, C.c_void_p, C.c_void_p)
     sig("ks_debug_update", i64, i64, i64, i32, i32, C.c_void_p, i32, f64, i64)
     sig("ks_debug_bwls_capture", i64, i32, i32, C.c_void_p, C.c_void_p)
+    sig("ks_debug_blockls_capture", i64, i32, i32, C.POINTER(C.c_void_p))
 
 
 def check(ctx: int, rc: int) -> None:

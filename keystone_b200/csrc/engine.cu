@@ -649,6 +649,17 @@ const GramTile* gram_tiles(Ctx& c, int b, int kcols, bool with_g, bool with_c, b
   return p;
 }
 
+// Rows of the contraction per Gram CTA: the length of one fp32 accumulation chain of the tensor core.  Every chunk ends in a
+// reduce-add of its 128 x 128 partial tile, so long chunks mean less reduce traffic and fewer, longer CTAs next to the critical
+// chain's kernels; short chunks keep enough CTAs per launch to balance the SMs when the rows are sharded (tools/ab_fit.py
+// compares settings).
+static int64_t gram_chain_rows(const Ctx& c, int64_t rows, bool f16, bool split, int64_t chunk_rows) {
+  const int stage_rows = split ? 32 : f16 ? 64 : kGramStageRows;
+  int64_t chunk = chunk_rows > 0 ? chunk_rows : c.gram_chunk_rows;
+  if (chunk <= 0) chunk = !f16 ? 4096 : rows >= 400000 ? 16384 : rows >= 200000 ? 8192 : 4096;
+  return std::max<int64_t>(stage_rows, chunk / stage_rows * stage_rows);
+}
+
 void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int b, const void* R, int64_t ldr, int kcols,
                        float* G, int ldg, float* C, int ldc, bool with_g, bool with_c, cudaStream_t st, bool f16,
                        int64_t chunk_rows, const void* slab_lo, const void* R_lo) {
@@ -681,13 +692,7 @@ void launch_gram_block(Ctx& c, const void* slab, int64_t lds, int64_t rows, int 
     else g.tmB1 = g.tmA;
   }
   g.rows = static_cast<int>(rows);
-  // Rows of the contraction per CTA.  Every chunk ends in a reduce-add of its 128 x 128 partial tile, so long chunks mean
-  // less reduce traffic and fewer, longer CTAs next to the critical chain's kernels; short chunks keep enough CTAs per
-  // launch to balance the SMs when the rows are sharded (tools/ab_fit.py compares settings).
-  int64_t chunk = chunk_rows > 0 ? chunk_rows : c.gram_chunk_rows;
-  if (chunk <= 0) chunk = !f16 ? 4096 : rows >= 400000 ? 16384 : rows >= 200000 ? 8192 : 4096;
-  chunk = std::max<int64_t>(stage_rows, chunk / stage_rows * stage_rows);
-  g.chunk_rows = static_cast<int>(chunk);
+  g.chunk_rows = static_cast<int>(gram_chain_rows(c, rows, f16, split, chunk_rows));
   if (with_g) tmap_or_throw(&g.tmOut0, G, b, b, ldg, 32);
   if (with_c) tmap_or_throw(&g.tmOut1, C, b, kcols, ldc, 32);
   if (!with_g) g.tmOut0 = g.tmOut1;
@@ -778,8 +783,8 @@ __global__ void sumsq_f64_kernel(const double* p, int64_t n, double* out) {
 // tensor kernels never share the SMs: each is written to own an SM (one CTA, ~200 KB of shared memory), so running two at
 // once only splits the machine, thrashes L2 and stretches both.
 // Slabs, G and H rotate through LA + 2 buffers; cross-stream dependencies are CUDA events; no host synchronisation inside the loop.
-static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double lam, int64_t nf_opt,
-                           int precision = KS_PRECISION_TF32) {
+static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter, double lam, int64_t nf_opt, int precision,
+                           const std::vector<Ctx::BlsCapture>& cap) {
   if (bs <= 0 || num_iter < 1) throw KsError{KS_ERR_INVALID, "blockSize must be > 0 and numIter >= 1"};
   if (Y.rows != src.n_rows) throw KsError{KS_ERR_INVALID, "features and labels have different row counts"};
   const int64_t n_loc = Y.rows;
@@ -961,6 +966,42 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
   int info_slot = 0;
   double flops = 0;
   const bool shard_solve = c.world > 1 && c.shard_solve && k >= c.world;
+  const int64_t chain_rows = gram_chain_rows(c, n_loc, f16, x2 && f16, x2 ? x2_chunk : 0);
+
+  // ---------------- ks_debug_blockls_capture: the host buffer step t requested for `what`, or null
+  auto cap_out = [&](int t, int what) -> double* {
+    for (const auto& q : cap)
+      if (q.sweep == steps[t].it && q.block == steps[t].j && q.out[what]) return q.out[what];
+    return nullptr;
+  };
+  // copies rows x cols elements (fp16, fp32 or fp64, leading dimension ld) once stream s has produced them, converted exactly to
+  // fp64; the host waits for s, which adds no work to any stream
+  auto cap_copy = [&](double* dst, const void* src_dev, int64_t rows, int64_t cols, int64_t ld, int elem, cudaStream_t s) {
+    if (!dst) return;
+    std::vector<unsigned char> h(static_cast<size_t>(elem) * static_cast<size_t>(std::max<int64_t>(rows, 1) * ld));
+    KS_CUDA(cudaMemcpyAsync(h.data(), src_dev, h.size(), cudaMemcpyDeviceToHost, s));
+    KS_CUDA(cudaStreamSynchronize(s));
+    for (int64_t r = 0; r < rows; ++r)
+      for (int64_t q = 0; q < cols; ++q) {
+        const size_t i = static_cast<size_t>(r * ld + q);
+        dst[r * cols + q] = elem == 2 ? static_cast<double>(__half2float(reinterpret_cast<const __half*>(h.data())[i]))
+                            : elem == 4 ? static_cast<double>(reinterpret_cast<const float*>(h.data())[i])
+                                        : reinterpret_cast<const double*>(h.data())[i];
+      }
+  };
+  auto cap_slab = [&](int t, int buf, int b) {  // the planes the Gram and update kernels read
+    cap_copy(cap_out(t, KS_BLS_CAP_SLAB_HI), slab[buf].p, n_loc, b, lds, static_cast<int>(es), ST);
+    if (double* lo = cap_out(t, KS_BLS_CAP_SLAB_LO)) {
+      if (x2) cap_copy(lo, slab_lo[buf].p, n_loc, b, lds, static_cast<int>(es), ST);
+      else std::fill(lo, lo + n_loc * b, 0.0);
+    }
+  };
+  auto cap_scales = [&](int t) {
+    if (double* d = cap_out(t, KS_BLS_CAP_SCALES)) {
+      if (f16) cap_copy(d, scales.as<float>() + 2, 1, 4, 4, 4, SS);
+      else std::fill(d, d + 4, 1.0);
+    }
+  };
 
 
   // ---------------- proj(t): shift estimate (first sweep) + slab of step t, on ST
@@ -999,6 +1040,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
         flops += 2.0 * static_cast<double>(ns) * src.d_in * b;
       }
     }
+    cap_copy(cap_out(t, KS_BLS_CAP_SHIFT), shifts[j]->p, 1, b, b, 4, ST);
     KS_CUDA(cudaMemsetAsync(ssum[buf].p, 0, ssum[buf].bytes, ST));
     float* cs = it == 0 ? ssum[buf].as<float>() : nullptr;
     if (x2 && src.F) {  // materialised features: tf32 hi / lo planes straight from F
@@ -1084,9 +1126,11 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     KS_CUDA(cudaStreamWaitEvent(SF, ev_g[t], 0));
     c.span_begin(PH_SOLVE, SF);
     launch_delta_mean(ssum[buf].as<float>(), shifts[j]->as<float>(), n_total_d, deltas[j]->as<double>(), model->mean[j]->as<double>(), b, SF);
+    if (x2) cap_copy(cap_out(t, KS_BLS_CAP_DIAG), dsq[buf].p, 1, b, b, 8, SF);
     launch_build_system(gbuf[buf].as<float>(), ldg, deltas[j]->as<double>(), n_total_d, lam, Hj, b, SF,
                         g_cross ? gbuf[buf].as<float>() + g_elems : nullptr, x2 ? dsq[buf].as<double>() : nullptr);
     c.launches += 2;
+    cap_copy(cap_out(t, KS_BLS_CAP_H), Hj, 1, static_cast<int64_t>(b) * b, static_cast<int64_t>(b) * b, 8, SF);
     c.potrf(Hj, b, info_slot++, SF);
     if (Dj) {  // inverses of the factor's 64 x 64 diagonal tiles: the in-tile substitutions of the solve become DMMA products
       KS_CUDA(launch_tri_inv_tiles(Hj, b, Dj, SF));
@@ -1102,6 +1146,8 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     const int j = steps[t].j, buf = t % NBUF;
     int64_t c0;
     const int b = block_cols(j, &c0);
+    cap_slab(t, buf, b);
+    cap_copy(cap_out(t, KS_BLS_CAP_R_BEFORE), r_f32.p, n_loc, k, kpad, 4, ST);
     c.span_begin(PH_OTHER, ST);
     KS_CUDA(cudaMemsetAsync(cm.p, 0, sizeof(float) * c_elems, ST));
     KS_CUDA(cudaMemsetAsync(rsum.p, 0, rsum.bytes, ST));
@@ -1146,6 +1192,8 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     launch_build_rhs(cm.as<float>(), ldc, deltas[j]->as<double>(), rsum.as<double>(), n_total_d, lam,
                      it > 0 ? model->W[j]->as<double>() : nullptr, rhs.as<double>(), b, k, SS, f16 ? rscale + 1 : nullptr);
     c.launches += 1;
+    cap_copy(cap_out(t, KS_BLS_CAP_DELTA), deltas[j]->p, 1, b, b, 8, SS);
+    cap_copy(cap_out(t, KS_BLS_CAP_RHS), rhs.p, 1, static_cast<int64_t>(b) * k, static_cast<int64_t>(b) * k, 8, SS);
     const double* Dj = !custom_solve ? nullptr : cache_factors ? dinvs[j]->as<double>() : Dbuf[buf].as<double>();
     auto solve_cols = [&](double* cols, int ncols) {  // (L L^T)^-1 on `ncols` right-hand sides, in place
       if (custom_solve) {
@@ -1172,6 +1220,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     } else {
       solve_cols(rhs.as<double>(), k);
     }
+    cap_copy(cap_out(t, KS_BLS_CAP_DW), rhs.p, 1, static_cast<int64_t>(b) * k, static_cast<int64_t>(b) * k, 8, SS);
     const double* dw_ptr = rhs.as<double>();
     if (f16) {
       KS_CUDA(cudaMemsetAsync(maxbits + 1, 0, sizeof(unsigned), SS));
@@ -1185,6 +1234,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
                          static_cast<int>(lds), cbias.as<float>(), b, k, static_cast<int>(kpad), SS);
     }
     c.launches += 1;
+    cap_scales(t);
     flops += 2.0 * static_cast<double>(b) * b * k;
     c.span_end(SS);
     KS_CUDA(cudaEventRecord(ev_solved[t], SS));
@@ -1217,6 +1267,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
     }
     flops += 2.0 * n_loc * static_cast<double>(b) * k;
     c.span_end(ST);
+    cap_copy(cap_out(t, KS_BLS_CAP_R_AFTER), r_f32.p, n_loc, k, kpad, 4, ST);
   };
 
   // Enqueue order: a stream-wait on an event that has not been recorded yet counts as complete, so every wait is enqueued
@@ -1275,7 +1326,7 @@ static int64_t fit_blockls(Ctx& c, FeatSrc& src, Matrix& Y, int bs, int num_iter
      << ",\"gram_ms\":" << ms[PH_GRAM] << ",\"allreduce_ms\":" << ms[PH_ALLREDUCE] << ",\"solve_ms\":" << ms[PH_SOLVE]
      << ",\"update_ms\":" << ms[PH_UPDATE] << ",\"other_ms\":" << ms[PH_OTHER] << ",\"local_flops\":" << flops
      << ",\"launches\":" << (c.launches - launches0) << ",\"mma\":\"" << (x2 ? (f16 ? "f16x2" : "tf32x2") : f16 ? "f16" : "tf32x1")
-     << "\",\"lookahead\":" << LA << ",\"host_mirror\":" << (model->host_valid ? 1 : 0) << ",\"solve\":\""
+     << "\",\"lookahead\":" << LA << ",\"chain_rows\":" << chain_rows << ",\"host_mirror\":" << (model->host_valid ? 1 : 0) << ",\"solve\":\""
      << (custom_solve ? "dmma-kernel" : "potrs") << (shard_solve ? "-column-sharded" : "") << "\",\"host_ms\":"
      << std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count() << "}";
   c.stats_json = js.str();
@@ -2012,11 +2063,13 @@ KS_API int32_t ks_blockls_fit(int64_t ctx, int64_t features, int64_t x_in, const
                        int32_t block_size, int32_t num_iter, double lambda, int64_t num_features_or_0, int32_t precision_mode,
                        int64_t* out_model) {
   return guard(ctx, [&](Ctx& c) {
+    std::vector<Ctx::BlsCapture> cap;  // ks_debug_blockls_capture arms one fit: take the requests and disarm before anything can throw
+    cap.swap(c.bls_cap);
     if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
     const int prec = resolve_precision(c, precision_mode);
     FeatSrc src;
     make_feat_src(c, features, x_in, rfs, n_rfs, src, prec);
-    *out_model = fit_blockls(c, src, c.matrix(labels), block_size, num_iter, lambda, num_features_or_0, prec);
+    *out_model = fit_blockls(c, src, c.matrix(labels), block_size, num_iter, lambda, num_features_or_0, prec, cap);
   });
 }
 
@@ -2109,12 +2162,15 @@ KS_API int32_t ks_naive_bayes_fit(int64_t ctx, int64_t features_or_0, int64_t sp
 
 KS_API int32_t ks_linear_map_fit(int64_t ctx, int64_t features, int64_t labels, int32_t has_lambda, double lambda, int64_t* out_model) {
   return guard(ctx, [&](Ctx& c) {
+    std::vector<Ctx::BlsCapture> cap;
+    cap.swap(c.bls_cap);
     if (!out_model) throw KsError{KS_ERR_INVALID, "null out_model"};
     FeatSrc src;
     make_feat_src(c, features, 0, nullptr, 0, src);
     // one block spanning every feature, one pass: exactly (A^T A [+ lambda I]) \ A^T y on centred data; the operand mode is the
     // context's ("precision" option; the default is the split-operand parity mode)
-    *out_model = fit_blockls(c, src, c.matrix(labels), static_cast<int>(src.D), 1, has_lambda ? lambda : 0.0, 0, c.precision);
+    *out_model = fit_blockls(c, src, c.matrix(labels), static_cast<int>(src.D), 1, has_lambda ? lambda : 0.0, 0, c.precision,
+                             cap);
   });
 }
 
@@ -2951,6 +3007,19 @@ KS_API int32_t ks_debug_bwls_capture(int64_t ctx, int32_t block, int32_t cls, do
     c.bwls_cap_cls = cls;
     c.bwls_cap_H = H_out;
     c.bwls_cap_rhs = rhs_out;
+  });
+}
+
+KS_API int32_t ks_debug_blockls_capture(int64_t ctx, int32_t sweep, int32_t block, double* const* outs) {
+  return guard(ctx, [&](Ctx& c) {
+    if (sweep < 0 || block < 0 || !outs) throw KsError{KS_ERR_INVALID, "bad arguments"};
+    if (sweep > 0 && (outs[KS_BLS_CAP_H] || outs[KS_BLS_CAP_DIAG]))
+      throw KsError{KS_ERR_INVALID, "H and the diagonal are assembled at sweep 0 only: later sweeps reuse the cached factor"};
+    Ctx::BlsCapture q;
+    q.sweep = sweep;
+    q.block = block;
+    std::copy(outs, outs + KS_BLS_CAP_COUNT, q.out);
+    c.bls_cap.push_back(q);
   });
 }
 

@@ -259,6 +259,12 @@ struct Ctx {
   int bwls_cap_block = -1, bwls_cap_cls = -1;
   double* bwls_cap_H = nullptr;
   double* bwls_cap_rhs = nullptr;
+  // ks_debug_blockls_capture: steps of the next block least-squares fit whose state is copied to host buffers (KS_BLS_CAP_*)
+  struct BlsCapture {
+    int sweep, block;
+    double* out[KS_BLS_CAP_COUNT];
+  };
+  std::vector<BlsCapture> bls_cap;
   void ensure_lanes(int n);
   // Cholesky factorisation of H (n x n, lower) + solve of nrhs right-hand sides in place, on lane q; status -> dev_info[slot]
   void lane_potrf_potrs(int q, double* H, int n, double* B, int nrhs, int info_slot);

@@ -463,7 +463,8 @@ def test_bwls_larger_problem_cosine_features(ctx):
     assert np.abs(pred - ref).max() < 5e-4
 
 
-@pytest.mark.parametrize("n,k", [(4096, 1000), (4096, 125), (4096, 250), (4096, 500), (300, 37), (128, 8), (5, 3), (1000, 1), (777, 130)])
+@pytest.mark.parametrize("n,k", [(4096, 1000), (4096, 125), (4096, 250), (4096, 500), (300, 37), (128, 8), (5, 3), (1000, 1), (777, 130),
+                                 (1000, 1057), (4096, 2000)])   # k > 8 * 132: chol_solve_kernel<16>
 def test_chol_solve_kernel(ctx, n, k):
     """The library's DMMA multi-RHS Cholesky solve (one launch; clusters of 2 / 4 / 8 CTAs per column group when there are few
     right-hand sides, as in the column-sharded multi-GPU solve) vs numpy, and vs cuSOLVER."""
