@@ -345,6 +345,8 @@ KS_API int32_t ks_lbfgs_fit(int64_t ctx, int64_t features, int64_t x_in, const i
 KS_API int32_t ks_sparse_from_host_csr(int64_t ctx, const int64_t* indptr, const int32_t* indices, const double* values, int64_t n_rows,
                                        int64_t n_cols, int64_t* out_s);
 KS_API int32_t ks_sparse_shape(int64_t ctx, int64_t s, int64_t* n_rows, int64_t* n_cols, int64_t* nnz);
+/* The CSR of s as stored (rows + 1 offsets, nnz column indices and values) into caller buffers. */
+KS_API int32_t ks_sparse_to_host_csr(int64_t ctx, int64_t s, int64_t* indptr, int32_t* indices, double* values);
 KS_API int32_t ks_sparse_destroy(int64_t ctx, int64_t s);
 /* Densify (K/nodes/util/Densify.scala): a new n_rows x n_cols fp32 matrix; repeated entries are summed in fp64 in upload order and
  * rounded once. */
@@ -382,6 +384,77 @@ KS_API int32_t ks_logistic_fit(int64_t ctx, int64_t features_or_0, int64_t spars
  * pi_c = log(n_c + lambda) - log(N + k lambda).  lambda finite and >= 0.  ks_last_fit_stats_json: solver "naive_bayes". */
 KS_API int32_t ks_naive_bayes_fit(int64_t ctx, int64_t features_or_0, int64_t sparse_or_0, const int32_t* labels, int64_t n_labels,
                                   int32_t num_classes, double lambda, int64_t* out_model);
+
+/* ---- the text front end (DESIGN.md section 23) ------------------------------------------------------------------------------------
+ * Trim, LowerCase, Tokenizer, NGramsFeaturizer, TermFrequency, CommonSparseFeatures / AllSparseFeatures, SparseFeatureVectorizer,
+ * HashingTF and NGramsHashingTF (K/nodes/nlp/StringUtils.scala, ngrams.scala, HashingTF.scala, NGramsHashingTF.scala,
+ * K/nodes/stats/TermFrequency.scala, K/nodes/util/{Common,All}SparseFeatures.scala, SparseFeatureVectorizer.scala).  Text objects
+ * (text, token and term-frequency batches, fitted feature spaces) share one handle space, released by ks_text_destroy; a text object
+ * keeps the objects it was made from alive.  Orders: (0, 0) takes every token as a term of its own (a Java String); 1 <= min <= max
+ * takes the n-grams of those orders (Scala Seqs of Strings), emitted per position i, then order.  Nothing here is collective. */
+#define KS_TEXT_TRIM 1   /* Java String.trim: strip leading and trailing code points <= U+0020 */
+#define KS_TEXT_LOWER 2  /* the one-to-one Unicode lowercase mapping per code point, U+0130 to U+0069 U+0307, no final-sigma rule */
+/* ks_ctx_set_option "debug_text_hash_bits" (1..64, for tests): the content hashes keep only their low bits, forcing collisions.  It
+ * is rejected once the context holds a text object, so that every object is hashed, sorted and looked up under one mask. */
+/* A batch of n_docs documents: bytes (n_bytes of UTF-8) and doc_offsets (n_docs + 1, from 0 to n_bytes, non-decreasing).  Invalid
+ * UTF-8 (a bad lead or continuation byte, an overlong form, a surrogate, a code point above U+10FFFF or a sequence that crosses a
+ * document boundary) is found on the device and rejected with KS_ERR_INVALID. */
+KS_API int32_t ks_text_from_host(int64_t ctx, const uint8_t* bytes, int64_t n_bytes, const int64_t* doc_offsets, int64_t n_docs,
+                                 int64_t* out_text);
+KS_API int32_t ks_text_transform(int64_t ctx, int64_t text, int32_t flags, int64_t* out_text);
+/* Tokenizer() (Java String.split on [\p{Punct}\s]+): a leading separator gives a leading "", trailing empty tokens are dropped, an
+ * empty document gives [""] and a document of separators only gives no token.  Per token the device also keeps Java's
+ * String.hashCode (over UTF-16 code units) and a 64-bit content hash. */
+KS_API int32_t ks_text_tokenize(int64_t ctx, int64_t text, int64_t* out_tokens);
+/* A token batch from the host: token t is bytes[token_offsets[t], token_offsets[t + 1]); document d holds tokens
+ * [doc_offsets[d], doc_offsets[d + 1]). */
+KS_API int32_t ks_tokens_from_host(int64_t ctx, const uint8_t* bytes, int64_t n_bytes, const int64_t* token_offsets, int64_t n_tokens,
+                                   const int64_t* doc_offsets, int64_t n_docs, int64_t* out_tokens);
+/* TermFrequency over the terms of a token batch (orders as above, max_order <= 4): per document its distinct terms in order of first
+ * occurrence, each with its count as value; *out_max_count is the largest count (0 without terms). */
+KS_API int32_t ks_term_frequency(int64_t ctx, int64_t tokens, int32_t min_order, int32_t max_order, int64_t* out_tf,
+                                 int64_t* out_max_count);
+/* value = table[count - 1] for every term (n >= the largest count, every entry finite) */
+KS_API int32_t ks_tf_set_weights(int64_t ctx, int64_t tf, const double* table, int64_t n);
+/* A term-frequency batch from the host over the tokens of a token batch: term e is tokens [term_first[e], term_first[e] + max(order, 1))
+ * of it, a String when term_order[e] is 0 and a Seq of term_order[e] <= 4 Strings otherwise, with value values[e] (finite);
+ * document d holds terms [doc_offsets[d], doc_offsets[d + 1]). */
+KS_API int32_t ks_tf_from_host(int64_t ctx, int64_t tokens, const int64_t* term_first, const int32_t* term_order, const double* values,
+                               int64_t n_terms, const int64_t* doc_offsets, int64_t n_docs, int64_t* out_tf);
+/* CommonSparseFeatures(num_features).fit, or AllSparseFeatures().fit with num_features = -1: the distinct terms ranked by the number of
+ * entries that hold them (document frequency), descending, then by their first entry; the first num_features of them.  Terms are the
+ * same feature exactly when their bytes are equal.  The space owns a copy of its terms.  KS_ERR_INVALID on a context with several
+ * ranks (an exact top-K over ranks is not implemented) and for a batch without terms (a space has at least one feature). */
+KS_API int32_t ks_sparse_features_fit(int64_t ctx, int64_t tf, int64_t num_features, int64_t* out_space);
+/* A feature space from the host: feature f (column f) is the term (term_first[f], term_order[f]) over the tokens of a token batch. */
+KS_API int32_t ks_sparse_features_from_host(int64_t ctx, int64_t tokens, const int64_t* term_first, const int32_t* term_order,
+                                            int64_t n_features, int64_t* out_space);
+/* SparseFeatureVectorizer.apply: a sparse matrix handle with one row per document and one column per feature, the value of every term
+ * found in the space by its bytes (others dropped), columns ascending and distinct within a row: a term an uploaded batch repeats
+ * within one document gives one entry, the sum of its values in entry order. */
+KS_API int32_t ks_sparse_features_apply(int64_t ctx, int64_t space, int64_t tf, int64_t* out_sparse);
+/* HashingTF(num_features) over the terms of a token batch (orders as above; no limit on max_order), which is NGramsHashingTF(orders,
+ * num_features) for orders >= 1: a sparse matrix handle of counts at column nonNegativeMod(term.##, num_features), String.hashCode for
+ * a String and MurmurHash3.seqHash for a Seq.  num_features in [1, INT32_MAX]. */
+KS_API int32_t ks_hashing_tf(int64_t ctx, int64_t tokens, int32_t min_order, int32_t max_order, int64_t num_features, int64_t* out_sparse);
+/* Host copies of a text object's arrays, for inspection.  KS_TEXT_BYTES (uint8): the UTF-8 the object's documents or tokens point
+ * into; KS_TEXT_DOC_OFFSETS (int64, documents + 1): byte offsets of a text batch, token offsets of a token batch, term offsets of a
+ * term-frequency batch; KS_TEXT_TOKEN_BEGIN / _END (int64): byte ranges of the tokens; KS_TEXT_TOKEN_JAVA_HASH (int32); KS_TEXT_TERM_FIRST
+ * (int64), _ORDER (int32), _COUNT (int32), _VALUE (double): the terms of a term-frequency batch or the features of a space.
+ * ks_text_array_size gives the element count (KS_ERR_INVALID: the object has no such array); ks_text_array copies n of them. */
+#define KS_TEXT_BYTES 0
+#define KS_TEXT_DOC_OFFSETS 1
+#define KS_TEXT_TOKEN_BEGIN 2
+#define KS_TEXT_TOKEN_END 3
+#define KS_TEXT_TOKEN_JAVA_HASH 4
+#define KS_TEXT_TERM_FIRST 5
+#define KS_TEXT_TERM_ORDER 6
+#define KS_TEXT_TERM_COUNT 7
+#define KS_TEXT_TERM_VALUE 8
+KS_API int32_t ks_text_array_size(int64_t ctx, int64_t obj, int32_t which, int64_t* out_n);
+KS_API int32_t ks_text_array(int64_t ctx, int64_t obj, int32_t which, void* out, int64_t n);
+KS_API int32_t ks_text_destroy(int64_t ctx, int64_t obj);
+
 
 /* ---- covariance-based transforms (DESIGN.md section 15) -------------------------------------
  * Every product of these fits runs in fp64 on the DMMA tensor core; they take no precision mode.  The fitted objects are ordinary

@@ -209,6 +209,189 @@ JFN(jlong, naiveBayesFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong
   if (p) env->ReleaseIntArrayElements(classes, p, JNI_ABORT);
   return ok(env, ctx, rc) ? h : 0;
 }
+// ---- the text front end (DESIGN.md section 23): documents and tokens arrive as UTF-8 bytes with int64 offsets; every handle is a
+// text object released by textDestroy, except the sparse matrices that sparseFeaturesApply / hashingTf return
+struct Bytes {  // borrowed view of a jbyteArray
+  JNIEnv* env;
+  jbyteArray arr;
+  jbyte* p = nullptr;
+  jsize n = 0;
+  Bytes(JNIEnv* e, jbyteArray a) : env(e), arr(a) {
+    if (arr) {
+      n = env->GetArrayLength(arr);
+      if (n) p = env->GetByteArrayElements(arr, nullptr);
+    }
+  }
+  ~Bytes() {
+    if (p) env->ReleaseByteArrayElements(arr, p, JNI_ABORT);
+  }
+  const uint8_t* data() const { return reinterpret_cast<const uint8_t*>(p); }
+};
+struct Ints {  // borrowed view of a jintArray
+  JNIEnv* env;
+  jintArray arr;
+  jint* p = nullptr;
+  jsize n = 0;
+  Ints(JNIEnv* e, jintArray a) : env(e), arr(a) {
+    if (arr) {
+      n = env->GetArrayLength(arr);
+      if (n) p = env->GetIntArrayElements(arr, nullptr);
+    }
+  }
+  ~Ints() {
+    if (p) env->ReleaseIntArrayElements(arr, p, JNI_ABORT);
+  }
+  const int32_t* data() const { return reinterpret_cast<const int32_t*>(p); }
+};
+struct Doubles {  // borrowed view of a jdoubleArray
+  JNIEnv* env;
+  jdoubleArray arr;
+  jdouble* p = nullptr;
+  jsize n = 0;
+  Doubles(JNIEnv* e, jdoubleArray a) : env(e), arr(a) {
+    if (arr) {
+      n = env->GetArrayLength(arr);
+      if (n) p = env->GetDoubleArrayElements(arr, nullptr);
+    }
+  }
+  ~Doubles() {
+    if (p) env->ReleaseDoubleArrayElements(arr, p, JNI_ABORT);
+  }
+};
+
+JFN(jlong, textFromHost)(JNIEnv* env, jobject, jlong ctx, jbyteArray bytes, jlongArray docOffsets) {
+  int64_t h = 0;
+  Bytes b(env, bytes);
+  LongArray off(env, docOffsets);
+  const int32_t rc = ks_text_from_host(ctx, b.data(), b.n, off.data(), off.n > 0 ? off.n - 1 : 0, &h);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, textTransform)(JNIEnv* env, jobject, jlong ctx, jlong text, jint flags) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_text_transform(ctx, text, flags, &h)) ? h : 0;
+}
+JFN(jlong, textTokenize)(JNIEnv* env, jobject, jlong ctx, jlong text) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_text_tokenize(ctx, text, &h)) ? h : 0;
+}
+JFN(jlong, tokensFromHost)(JNIEnv* env, jobject, jlong ctx, jbyteArray bytes, jlongArray tokenOffsets, jlongArray docOffsets) {
+  int64_t h = 0;
+  Bytes b(env, bytes);
+  LongArray toff(env, tokenOffsets), doff(env, docOffsets);
+  const int32_t rc = ks_tokens_from_host(ctx, b.data(), b.n, toff.data(), toff.n > 0 ? toff.n - 1 : 0, doff.data(), doff.n > 0 ? doff.n - 1 : 0, &h);
+  return ok(env, ctx, rc) ? h : 0;
+}
+// returns (term-frequency handle, largest count)
+JFN(jlongArray, termFrequency)(JNIEnv* env, jobject, jlong ctx, jlong tokens, jint minOrder, jint maxOrder) {
+  int64_t h = 0, mc = 0;
+  if (!ok(env, ctx, ks_term_frequency(ctx, tokens, minOrder, maxOrder, &h, &mc))) return nullptr;
+  jlongArray out = env->NewLongArray(2);
+  if (!out) return nullptr;
+  const jlong v[2] = {h, mc};
+  env->SetLongArrayRegion(out, 0, 2, v);
+  return out;
+}
+JFN(void, tfSetWeights)(JNIEnv* env, jobject, jlong ctx, jlong tf, jdoubleArray table) {
+  Doubles t(env, table);
+  ok(env, ctx, ks_tf_set_weights(ctx, tf, t.p, t.n));
+}
+JFN(jlong, tfFromHost)(JNIEnv* env, jobject, jlong ctx, jlong tokens, jlongArray termFirst, jintArray termOrder, jdoubleArray values,
+                       jlongArray docOffsets) {
+  int64_t h = 0;
+  LongArray first(env, termFirst), doff(env, docOffsets);
+  Ints order(env, termOrder);
+  Doubles v(env, values);
+  const int32_t rc = ks_tf_from_host(ctx, tokens, first.data(), order.data(), v.p, first.n, doff.data(), doff.n > 0 ? doff.n - 1 : 0, &h);
+  return ok(env, ctx, rc) ? h : 0;
+}
+JFN(jlong, sparseFeaturesFit)(JNIEnv* env, jobject, jlong ctx, jlong tf, jlong numFeatures) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_sparse_features_fit(ctx, tf, numFeatures, &h)) ? h : 0;
+}
+JFN(jlong, sparseFeaturesFromHost)(JNIEnv* env, jobject, jlong ctx, jlong tokens, jlongArray termFirst, jintArray termOrder) {
+  int64_t h = 0;
+  LongArray first(env, termFirst);
+  Ints order(env, termOrder);
+  return ok(env, ctx, ks_sparse_features_from_host(ctx, tokens, first.data(), order.data(), first.n, &h)) ? h : 0;
+}
+JFN(jlong, sparseFeaturesApply)(JNIEnv* env, jobject, jlong ctx, jlong space, jlong tf) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_sparse_features_apply(ctx, space, tf, &h)) ? h : 0;
+}
+JFN(jlong, hashingTf)(JNIEnv* env, jobject, jlong ctx, jlong tokens, jint minOrder, jint maxOrder, jlong numFeatures) {
+  int64_t h = 0;
+  return ok(env, ctx, ks_hashing_tf(ctx, tokens, minOrder, maxOrder, numFeatures, &h)) ? h : 0;
+}
+// a text object's array `which` (KS_TEXT_*) as bytes, ints, longs or doubles, whichever its element type is
+static jsize text_array_size(JNIEnv* env, jlong ctx, jlong obj, jint which, bool* good) {
+  int64_t n = 0;
+  *good = ok(env, ctx, ks_text_array_size(ctx, obj, which, &n));
+  return static_cast<jsize>(n);
+}
+JFN(jbyteArray, textArrayBytes)(JNIEnv* env, jobject, jlong ctx, jlong obj, jint which) {
+  bool good;
+  const jsize n = text_array_size(env, ctx, obj, which, &good);
+  if (!good) return nullptr;
+  std::vector<jbyte> v(n);
+  if (!ok(env, ctx, ks_text_array(ctx, obj, which, v.data(), n))) return nullptr;
+  jbyteArray out = env->NewByteArray(n);
+  if (out) env->SetByteArrayRegion(out, 0, n, v.data());
+  return out;
+}
+JFN(jintArray, textArrayInts)(JNIEnv* env, jobject, jlong ctx, jlong obj, jint which) {
+  bool good;
+  const jsize n = text_array_size(env, ctx, obj, which, &good);
+  if (!good) return nullptr;
+  std::vector<jint> v(n);
+  if (!ok(env, ctx, ks_text_array(ctx, obj, which, v.data(), n))) return nullptr;
+  jintArray out = env->NewIntArray(n);
+  if (out) env->SetIntArrayRegion(out, 0, n, v.data());
+  return out;
+}
+JFN(jlongArray, textArrayLongs)(JNIEnv* env, jobject, jlong ctx, jlong obj, jint which) {
+  bool good;
+  const jsize n = text_array_size(env, ctx, obj, which, &good);
+  if (!good) return nullptr;
+  std::vector<jlong> v(n);
+  if (!ok(env, ctx, ks_text_array(ctx, obj, which, v.data(), n))) return nullptr;
+  jlongArray out = env->NewLongArray(n);
+  if (out) env->SetLongArrayRegion(out, 0, n, v.data());
+  return out;
+}
+JFN(jdoubleArray, textArrayDoubles)(JNIEnv* env, jobject, jlong ctx, jlong obj, jint which) {
+  bool good;
+  const jsize n = text_array_size(env, ctx, obj, which, &good);
+  if (!good) return nullptr;
+  std::vector<jdouble> v(n);
+  if (!ok(env, ctx, ks_text_array(ctx, obj, which, v.data(), n))) return nullptr;
+  jdoubleArray out = env->NewDoubleArray(n);
+  if (out) env->SetDoubleArrayRegion(out, 0, n, v.data());
+  return out;
+}
+JFN(void, textDestroy)(JNIEnv*, jobject, jlong ctx, jlong obj) { ks_text_destroy(ctx, obj); }
+// a sparse matrix as (indptr, indices, values); the Scala side turns row r into a SparseVector
+JFN(jobjectArray, sparseToHostCsr)(JNIEnv* env, jobject, jlong ctx, jlong s) {  // [long[] indptr, int[] indices, double[] values]
+  int64_t rows = 0, cols = 0, nnz = 0;
+  if (!ok(env, ctx, ks_sparse_shape(ctx, s, &rows, &cols, &nnz))) return nullptr;
+  std::vector<int64_t> ip(rows + 1);
+  std::vector<int32_t> ix(nnz);
+  std::vector<double> v(nnz);
+  if (!ok(env, ctx, ks_sparse_to_host_csr(ctx, s, ip.data(), ix.data(), v.data()))) return nullptr;
+  jclass objc = env->FindClass("java/lang/Object");
+  if (!objc) return nullptr;
+  jobjectArray out = env->NewObjectArray(3, objc, nullptr);
+  jlongArray a = env->NewLongArray(static_cast<jsize>(rows + 1));
+  jintArray b = env->NewIntArray(static_cast<jsize>(nnz));
+  jdoubleArray d = env->NewDoubleArray(static_cast<jsize>(nnz));
+  if (!out || !a || !b || !d) return nullptr;
+  env->SetLongArrayRegion(a, 0, static_cast<jsize>(rows + 1), reinterpret_cast<const jlong*>(ip.data()));
+  env->SetIntArrayRegion(b, 0, static_cast<jsize>(nnz), ix.data());
+  env->SetDoubleArrayRegion(d, 0, static_cast<jsize>(nnz), v.data());
+  env->SetObjectArrayElement(out, 0, a);
+  env->SetObjectArrayElement(out, 1, b);
+  env->SetObjectArrayElement(out, 2, d);
+  return out;
+}
 JFN(jlong, linearMapFit)(JNIEnv* env, jobject, jlong ctx, jlong features, jlong labels, jboolean hasLambda, jdouble lambda) {
   int64_t h = 0;
   return ok(env, ctx, ks_linear_map_fit(ctx, features, labels, hasLambda ? 1 : 0, lambda, &h)) ? h : 0;

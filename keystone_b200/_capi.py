@@ -19,6 +19,9 @@ KS_PRECISION_TF32 = 0
 KS_PRECISION_F16 = 1
 KS_PRECISION_F16X2 = 2  # split-operand parity mode
 KS_PRECISION_DEFAULT = -1
+KS_TEXT_TRIM, KS_TEXT_LOWER = 1, 2
+(KS_TEXT_BYTES, KS_TEXT_DOC_OFFSETS, KS_TEXT_TOKEN_BEGIN, KS_TEXT_TOKEN_END, KS_TEXT_TOKEN_JAVA_HASH, KS_TEXT_TERM_FIRST, KS_TEXT_TERM_ORDER,
+ KS_TEXT_TERM_COUNT, KS_TEXT_TERM_VALUE) = range(9)
 PRECISIONS = {"tf32": KS_PRECISION_TF32, "f16": KS_PRECISION_F16, "f16x2": KS_PRECISION_F16X2, "parity": KS_PRECISION_F16X2,
               "default": KS_PRECISION_DEFAULT}
 
@@ -115,12 +118,27 @@ def _declare(L: C.CDLL) -> None:
     sig("ks_lbfgs_fit", i64, i64, i64, p_i64, i32, i64, i32, i32, f64, i32, f64, i32, p_i64)
     sig("ks_sparse_from_host_csr", i64, C.c_void_p, C.c_void_p, C.c_void_p, i64, i64, p_i64)
     sig("ks_sparse_shape", i64, i64, p_i64, p_i64, p_i64)
+    sig("ks_sparse_to_host_csr", i64, i64, C.c_void_p, C.c_void_p, C.c_void_p)
     sig("ks_sparse_destroy", i64, i64)
     sig("ks_sparse_densify", i64, i64, p_i64)
     sig("ks_sparse_lbfgs_fit", i64, i64, i64, i32, i32, f64, i32, f64, p_i64)
     sig("ks_model_apply_sparse", i64, i64, i64, p_i64)
     sig("ks_logistic_fit", i64, i64, i64, C.c_void_p, i64, i32, f64, i32, f64, p_i64)
     sig("ks_naive_bayes_fit", i64, i64, i64, C.c_void_p, i64, i32, f64, p_i64)
+    sig("ks_text_from_host", i64, C.c_void_p, i64, C.c_void_p, i64, p_i64)
+    sig("ks_text_transform", i64, i64, i32, p_i64)
+    sig("ks_text_tokenize", i64, i64, p_i64)
+    sig("ks_tokens_from_host", i64, C.c_void_p, i64, C.c_void_p, i64, C.c_void_p, i64, p_i64)
+    sig("ks_term_frequency", i64, i64, i32, i32, p_i64, p_i64)
+    sig("ks_tf_set_weights", i64, i64, C.c_void_p, i64)
+    sig("ks_tf_from_host", i64, i64, C.c_void_p, C.c_void_p, C.c_void_p, i64, C.c_void_p, i64, p_i64)
+    sig("ks_sparse_features_fit", i64, i64, i64, p_i64)
+    sig("ks_sparse_features_from_host", i64, i64, C.c_void_p, C.c_void_p, i64, p_i64)
+    sig("ks_sparse_features_apply", i64, i64, i64, p_i64)
+    sig("ks_hashing_tf", i64, i64, i32, i32, i64, p_i64)
+    sig("ks_text_array_size", i64, i64, i32, p_i64)
+    sig("ks_text_array", i64, i64, i32, C.c_void_p, i64)
+    sig("ks_text_destroy", i64, i64)
     sig("ks_pca_fit", i64, i64, i32, p_i64)
     sig("ks_zca_fit", i64, i64, f64, p_i64)
     sig("ks_approx_range", i64, i64, C.c_void_p, i32, i32, p_i64)

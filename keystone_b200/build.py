@@ -15,8 +15,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libkeystone_b200.so")
-SOURCES = ["tc_kernels.cu", "aux_kernels.cu", "solve_kernels.cu", "engine.cu", "bwls.cu", "krr.cu", "lbfgs.cu", "sparse.cu", "logistic.cu", "pca.cu", "fisher.cu", "gmm_fit.cu", "sift.cu", "hog_daisy.cu", "augment.cu", "io.cu"]
-HEADERS = ["tc_common.cuh", "cluster.cuh", "kernels.h", "operand_split.cuh", "lbfgs_core.cuh", "engine.h", os.path.join("..", "..", "include", "keystone_b200.h")]
+SOURCES = ["tc_kernels.cu", "aux_kernels.cu", "solve_kernels.cu", "engine.cu", "bwls.cu", "krr.cu", "lbfgs.cu", "sparse.cu", "logistic.cu", "pca.cu", "fisher.cu", "gmm_fit.cu", "sift.cu", "hog_daisy.cu", "augment.cu", "text.cu", "io.cu"]
+HEADERS = ["tc_common.cuh", "cluster.cuh", "kernels.h", "operand_split.cuh", "lbfgs_core.cuh", "lower_table.h", "engine.h", os.path.join("..", "..", "include", "keystone_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "-DKS_BUILD",

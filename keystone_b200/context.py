@@ -165,6 +165,41 @@ class Context:
                                                           data.ctypes.data_as(C.c_void_p), n_rows, n_cols, C.byref(h)))
         return SparseMatrix(self, h.value, n_rows, n_cols, nnz)
 
+    def text(self, docs: Sequence) -> "TextBatch":
+        """A batch of documents on the device (``ks_text_from_host``): each ``str`` is encoded as UTF-8 (a lone surrogate is
+        rejected here); ``bytes`` items are taken as they are, and invalid UTF-8 among them is found on the device and rejected."""
+        data, off = _encode_all(docs, "document")
+        h = C.c_int64(0)
+        check(self.handle, lib().ks_text_from_host(self.handle, data.ctypes.data_as(C.c_void_p), data.shape[0], off.ctypes.data_as(C.c_void_p),
+                                                    off.shape[0] - 1, C.byref(h)))
+        return TextBatch(self, h.value, off.shape[0] - 1)
+
+    def tokens(self, docs: Sequence[Sequence[str]]) -> "TokenBatch":
+        """A token batch from host lists of strings, one list per document (``ks_tokens_from_host``)."""
+        flat = [t for d in docs for t in d]
+        data, toff = _encode_all(flat, "token")
+        doff = np.zeros(len(docs) + 1, dtype=np.int64)
+        doff[1:] = np.cumsum([len(d) for d in docs])
+        h = C.c_int64(0)
+        check(self.handle, lib().ks_tokens_from_host(self.handle, data.ctypes.data_as(C.c_void_p), data.shape[0], toff.ctypes.data_as(C.c_void_p),
+                                                      len(flat), doff.ctypes.data_as(C.c_void_p), len(docs), C.byref(h)))
+        return TokenBatch(self, h.value, len(docs))
+
+    def term_frequencies(self, docs: Sequence[Sequence[tuple]]) -> "TermFrequencyBatch":
+        """A term-frequency batch from host lists of ``(term, value)`` pairs, one list per document: a term is a ``str`` or a tuple
+        of one to four ``str`` (``ks_tf_from_host``)."""
+        terms = [t for d in docs for t, _ in d]
+        tokens, first, order = _flatten_terms(terms)
+        values = np.ascontiguousarray([float(v) for d in docs for _, v in d], dtype=np.float64)
+        doff = np.zeros(len(docs) + 1, dtype=np.int64)
+        doff[1:] = np.cumsum([len(d) for d in docs])
+        tk = self.tokens([tokens])
+        h = C.c_int64(0)
+        check(self.handle, lib().ks_tf_from_host(self.handle, tk.handle, first.ctypes.data_as(C.c_void_p), order.ctypes.data_as(C.c_void_p),
+                                                  values.ctypes.data_as(C.c_void_p), len(terms), doff.ctypes.data_as(C.c_void_p), len(docs),
+                                                  C.byref(h)))
+        return TermFrequencyBatch(self, h.value, len(docs), tk)
+
     def labels_from_classes(self, classes: np.ndarray, num_classes: int) -> "DeviceMatrix":
         cls = np.ascontiguousarray(classes, dtype=np.int32)
         h = C.c_int64(0)
@@ -215,6 +250,15 @@ class SparseMatrix(Dataset):
     @property
     def shape(self):
         return (self.rows, self.cols)
+
+    def to_csr(self):
+        """(indptr int64, indices int32, data fp64) of this rank's rows as stored on the device."""
+        indptr = np.empty(self.rows + 1, dtype=np.int64)
+        indices = np.empty(self.nnz, dtype=np.int32)
+        data = np.empty(self.nnz, dtype=np.float64)
+        check(self.ctx.handle, lib().ks_sparse_to_host_csr(self.ctx.handle, self.handle, indptr.ctypes.data_as(C.c_void_p),
+                                                            indices.ctypes.data_as(C.c_void_p), data.ctypes.data_as(C.c_void_p)))
+        return indptr, indices, data
 
     def free(self) -> None:
         if self.handle and self.ctx.handle:
@@ -279,3 +323,143 @@ def feature_source_args(data: Dataset):
         arr = (C.c_int64 * len(data.rf_handles))(*data.rf_handles)
         return 0, data.x_in.handle, arr, len(data.rf_handles)
     raise KeystoneError(-1, f"unsupported dataset type {type(data).__name__}")
+
+
+# ---- text batches (text.cu, DESIGN.md section 23) ----
+def _encode_all(items: Sequence, what: str):
+    """(uint8 bytes, int64 offsets) of the UTF-8 encodings of ``items`` (``str`` or ``bytes``)."""
+    parts = []
+    for i, x in enumerate(items):
+        if isinstance(x, (bytes, bytearray)):
+            parts.append(bytes(x))
+        elif isinstance(x, str):
+            try:
+                parts.append(x.encode("utf-8"))
+            except UnicodeEncodeError as e:
+                raise KeystoneError(-1, f"{what} {i} holds a lone surrogate (U+{ord(x[e.start]):04X}), which has no UTF-8 form") from None
+        else:
+            raise KeystoneError(-1, f"{what} {i} is a {type(x).__name__}, not a str")
+    off = np.zeros(len(parts) + 1, dtype=np.int64)
+    off[1:] = np.cumsum([len(p) for p in parts])
+    data = np.frombuffer(b"".join(parts), dtype=np.uint8) if parts else np.zeros(0, dtype=np.uint8)
+    return np.ascontiguousarray(data), off
+
+
+def _flatten_terms(terms: Sequence):
+    """Terms (``str``, or tuples of one to four ``str``) as (tokens, first token, order): order 0 marks a ``str``."""
+    tokens: List[str] = []
+    first = np.zeros(len(terms), dtype=np.int64)
+    order = np.zeros(len(terms), dtype=np.int32)
+    for i, t in enumerate(terms):
+        first[i] = len(tokens)
+        if isinstance(t, str):
+            tokens.append(t)
+        elif isinstance(t, tuple) and 1 <= len(t) <= 4 and all(isinstance(w, str) for w in t):
+            tokens.extend(t)
+            order[i] = len(t)
+        else:
+            raise KeystoneError(-1, f"term {t!r}: a term on the device is a str or a tuple of one to four str")
+    return tokens, first, order
+
+
+def _text_array(ctx: Context, handle: int, which: int, dtype) -> np.ndarray:
+    n = C.c_int64(0)
+    check(ctx.handle, lib().ks_text_array_size(ctx.handle, handle, which, C.byref(n)))
+    out = np.empty(n.value, dtype=dtype)
+    check(ctx.handle, lib().ks_text_array(ctx.handle, handle, which, out.ctypes.data_as(C.c_void_p), n.value))
+    return out
+
+
+def _host_tokens(ctx: Context, handle: int) -> List[str]:
+    data = _text_array(ctx, handle, _capi.KS_TEXT_BYTES, np.uint8).tobytes()
+    tb = _text_array(ctx, handle, _capi.KS_TEXT_TOKEN_BEGIN, np.int64)
+    te = _text_array(ctx, handle, _capi.KS_TEXT_TOKEN_END, np.int64)
+    return [data[a:b].decode("utf-8") for a, b in zip(tb.tolist(), te.tolist())]
+
+
+def _host_terms(ctx: Context, handle: int) -> list:
+    toks = _host_tokens(ctx, handle)
+    first = _text_array(ctx, handle, _capi.KS_TEXT_TERM_FIRST, np.int64).tolist()
+    order = _text_array(ctx, handle, _capi.KS_TEXT_TERM_ORDER, np.int32).tolist()
+    return [toks[f] if o == 0 else tuple(toks[f:f + o]) for f, o in zip(first, order)]
+
+
+class _TextObject(Dataset):
+    def __init__(self, ctx: Context, handle: int, n_docs: int):
+        self.ctx, self.handle, self.n_docs = ctx, handle, n_docs
+
+    def __len__(self):
+        return self.n_docs
+
+    def free(self) -> None:
+        if self.handle and self.ctx.handle:
+            lib().ks_text_destroy(self.ctx.handle, self.handle)
+        self.handle = 0
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class TextBatch(_TextObject):
+    """This rank's documents on the device: UTF-8 bytes and int64 document offsets (the reference's ``RDD[String]``)."""
+
+    def to_host(self) -> List[str]:
+        data = _text_array(self.ctx, self.handle, _capi.KS_TEXT_BYTES, np.uint8).tobytes()
+        off = _text_array(self.ctx, self.handle, _capi.KS_TEXT_DOC_OFFSETS, np.int64).tolist()
+        return [data[off[d]:off[d + 1]].decode("utf-8") for d in range(self.n_docs)]
+
+
+class TokenBatch(_TextObject):
+    """The tokens of each document (``RDD[Seq[String]]``): byte ranges into the text they came from, with Java's
+    ``String.hashCode`` and a content hash of each."""
+
+    def to_host(self) -> List[List[str]]:
+        toks = _host_tokens(self.ctx, self.handle)
+        off = _text_array(self.ctx, self.handle, _capi.KS_TEXT_DOC_OFFSETS, np.int64).tolist()
+        return [toks[off[d]:off[d + 1]] for d in range(self.n_docs)]
+
+    def java_hashes(self) -> np.ndarray:
+        """``String.hashCode`` of every token, in order (int32)."""
+        return _text_array(self.ctx, self.handle, _capi.KS_TEXT_TOKEN_JAVA_HASH, np.int32)
+
+
+class NGramBatch(Dataset):
+    """The n-grams of the given orders of a token batch (``RDD[Seq[Seq[String]]]``), lazy: the device emits them inside the node
+    that consumes them.  Per document they come in ``NGramsFeaturizer``'s order: for each position, each order ascending."""
+
+    def __init__(self, tokens: TokenBatch, min_order: int, max_order: int):
+        self.ctx, self.tokens, self.min_order, self.max_order = tokens.ctx, tokens, int(min_order), int(max_order)
+        self.n_docs = tokens.n_docs
+
+    def __len__(self):
+        return self.n_docs
+
+    def to_host(self) -> List[List[tuple]]:
+        out = []
+        for toks in self.tokens.to_host():
+            grams = []
+            for i in range(len(toks) - self.min_order + 1):
+                for o in range(self.min_order, self.max_order + 1):
+                    if i + o > len(toks):
+                        break
+                    grams.append(tuple(toks[i:i + o]))
+            out.append(grams)
+        return out
+
+
+class TermFrequencyBatch(_TextObject):
+    """Per document its distinct terms with a value (``RDD[Seq[(T, Double)]]``); ``max_count`` is the largest count in the batch
+    (0 for an uploaded batch, which carries values only)."""
+
+    def __init__(self, ctx: Context, handle: int, n_docs: int, tokens: Dataset, max_count: int = 0):
+        super().__init__(ctx, handle, n_docs)
+        self.tokens, self.max_count = tokens, int(max_count)
+
+    def to_host(self) -> List[List[tuple]]:
+        terms = _host_terms(self.ctx, self.handle)
+        values = _text_array(self.ctx, self.handle, _capi.KS_TEXT_TERM_VALUE, np.float64).tolist()
+        off = _text_array(self.ctx, self.handle, _capi.KS_TEXT_DOC_OFFSETS, np.int64).tolist()
+        return [list(zip(terms[off[d]:off[d + 1]], values[off[d]:off[d + 1]])) for d in range(self.n_docs)]

@@ -1463,6 +1463,8 @@ static int32_t guard(int64_t ctx, Fn&& fn) {
   }
 }
 
+int32_t ks::guarded(int64_t ctx, const std::function<void(Ctx&)>& fn) { return guard(ctx, fn); }
+
 extern "C" {
 
 KS_API int32_t ks_version(void) { return 100; }
@@ -1615,6 +1617,11 @@ KS_API int32_t ks_ctx_set_option(int64_t ctx, const char* name, int64_t value) {
     else if (n == "lookahead" && value >= 0 && value <= 6) c.lookahead = static_cast<int>(value);
     else if (n == "solve_lanes" && value >= 1 && value <= 16) c.solve_lanes = static_cast<int>(value);
     else if (n == "host_mirror") c.host_mirror = value != 0;
+    else if (n == "debug_text_hash_bits" && value >= 1 && value <= 64) {
+      // every text object's hashes, sorts and lookups must use one mask: the option is fixed once a text object exists
+      if (!c.texts.empty()) throw KsError{KS_ERR_INVALID, "debug_text_hash_bits must be set before any text object is created"};
+      c.text_hash_bits = static_cast<int>(value);
+    }
     else throw KsError{KS_ERR_INVALID, "unknown option or bad value: " + n};
   });
 }
@@ -2115,6 +2122,18 @@ KS_API int32_t ks_sparse_shape(int64_t ctx, int64_t s, int64_t* n_rows, int64_t*
     if (n_rows) *n_rows = sm.rows;
     if (n_cols) *n_cols = sm.cols;
     if (nnz) *nnz = sm.nnz;
+  });
+}
+KS_API int32_t ks_sparse_to_host_csr(int64_t ctx, int64_t s, int64_t* indptr, int32_t* indices, double* values) {
+  return guard(ctx, [&](Ctx& c) {
+    SparseMat& sm = c.sparse(s);
+    if (!indptr || (sm.nnz > 0 && (!indices || !values))) throw KsError{KS_ERR_INVALID, "null output"};
+    KS_CUDA(cudaMemcpyAsync(indptr, sm.indptr.p, sizeof(int64_t) * (sm.rows + 1), cudaMemcpyDeviceToHost, c.st));
+    if (sm.nnz > 0) {
+      KS_CUDA(cudaMemcpyAsync(indices, sm.indices.p, sizeof(int32_t) * sm.nnz, cudaMemcpyDeviceToHost, c.st));
+      KS_CUDA(cudaMemcpyAsync(values, sm.values.p, sizeof(double) * sm.nnz, cudaMemcpyDeviceToHost, c.st));
+    }
+    KS_CUDA(cudaStreamSynchronize(c.st));
   });
 }
 KS_API int32_t ks_sparse_destroy(int64_t ctx, int64_t s) {

@@ -5,6 +5,7 @@
 #include <nccl.h>
 #include <stdint.h>
 
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -179,6 +180,8 @@ struct SparseMat {
   SpTable rowt, colt;
 };
 
+struct TextObj;  // text batches, token batches, term frequencies and fitted feature spaces (text.cu, DESIGN.md section 23)
+
 struct SolverApi {
   void* lib = nullptr;
   cusolverStatus_t (*Create)(cusolverDnHandle_t*) = nullptr;
@@ -292,6 +295,8 @@ struct Ctx {
   std::unordered_map<int64_t, std::shared_ptr<GaussKernel>> kernels;
   std::unordered_map<int64_t, std::unique_ptr<Gmm>> gmms;
   std::unordered_map<int64_t, std::unique_ptr<SparseMat>> sparses;
+  std::unordered_map<int64_t, std::shared_ptr<TextObj>> texts;
+  int text_hash_bits = 64;  // bits kept of the 64-bit content hashes of text.cu (a test lowers it to force collisions)
   std::map<std::vector<int>, std::unique_ptr<DevBuf>> tile_cache;
   // phase timing of the current fit
   struct Span { int phase; cudaEvent_t a, b; int stream; };
@@ -512,6 +517,9 @@ void grouped_confusion_matrix(Ctx& c, Matrix& scores, const int64_t* rows, const
 // Sparse matrices (sparse.cu); none of these is collective
 std::unique_ptr<SparseMat> sparse_from_host_csr(Ctx& c, const int64_t* indptr, const int32_t* indices, const double* values, int64_t n_rows,
                                                 int64_t n_cols);
+// the rest of an upload for a CSR already on the device (s: rows, cols, nnz, indptr, indices, values set): the checks of
+// sparse_from_host_csr on the entries, the CSC copy and the work tables.  host_indptr_or_null: a host copy of indptr, if there is one.
+std::unique_ptr<SparseMat> sparse_from_device_csr(Ctx& c, std::unique_ptr<SparseMat> s, const int64_t* host_indptr_or_null);
 // out (lines x k, row-major fp64) = A X (transpose = false: lines = rows, X is cols x k) or A^T X (transpose = true: lines = cols,
 // X is rows x k), X row-major with ld k; bias_or_null (k values) is added to every line.  Fixed summation order.
 void sparse_product(Ctx& c, const SparseMat& s, bool transpose, const double* X, int k, const double* bias_or_null, double* out,
@@ -529,5 +537,9 @@ int64_t fit_sparse_lbfgs(Ctx& c, const SparseMat& s, Matrix& Y, bool fit_interce
 int64_t fit_logistic(Ctx& c, int64_t features, int64_t sparse, const int32_t* labels, int64_t n_labels, int num_classes, double reg_param,
                      int num_iterations, double convergence_tol);
 int64_t fit_naive_bayes(Ctx& c, int64_t features, int64_t sparse, const int32_t* labels, int64_t n_labels, int num_classes, double lambda);
+
+// runs fn on the context ctx as every C ABI entry does: KS_ERR_HANDLE for an unknown context, a thrown KsError becomes its code and
+// ks_last_error's message (engine.cu)
+int32_t guarded(int64_t ctx, const std::function<void(Ctx&)>& fn);
 
 }  // namespace ks

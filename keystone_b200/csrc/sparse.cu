@@ -10,6 +10,7 @@
 
 #include <cub/device/device_radix_sort.cuh>
 
+#include <algorithm>
 #include <cmath>
 #include <limits>
 #include <vector>
@@ -118,6 +119,12 @@ std::unique_ptr<SparseMat> sparse_from_host_csr(Ctx& c, const int64_t* indptr, c
     KS_CUDA(cudaMemcpyAsync(s->indices.p, indices, sizeof(int32_t) * nnz, cudaMemcpyHostToDevice, st));
     KS_CUDA(cudaMemcpyAsync(s->values.p, values, sizeof(double) * nnz, cudaMemcpyHostToDevice, st));
   }
+  return sparse_from_device_csr(c, std::move(s), indptr);
+}
+
+std::unique_ptr<SparseMat> sparse_from_device_csr(Ctx& c, std::unique_ptr<SparseMat> s, const int64_t* host_indptr_or_null) {
+  cudaStream_t st = c.st;
+  const int64_t n_rows = s->rows, n_cols = s->cols, nnz = s->nnz;
   DevBuf flag;
   flag.alloc(sizeof(unsigned));
   KS_CUDA(cudaMemsetAsync(flag.p, 0, sizeof(unsigned), st));
@@ -160,7 +167,14 @@ std::unique_ptr<SparseMat> sparse_from_host_csr(Ctx& c, const int64_t* indptr, c
   std::vector<int64_t> colptr(static_cast<size_t>(n_cols + 1));
   KS_CUDA(cudaMemcpyAsync(colptr.data(), s->colptr.p, sizeof(int64_t) * (n_cols + 1), cudaMemcpyDeviceToHost, st));
   KS_CUDA(cudaStreamSynchronize(st));
-  build_table(std::vector<int64_t>(indptr, indptr + n_rows + 1), n_rows, s->rowt, st);
+  std::vector<int64_t> indptr(static_cast<size_t>(n_rows + 1));
+  if (host_indptr_or_null) {
+    std::copy(host_indptr_or_null, host_indptr_or_null + n_rows + 1, indptr.begin());
+  } else {
+    KS_CUDA(cudaMemcpyAsync(indptr.data(), s->indptr.p, sizeof(int64_t) * (n_rows + 1), cudaMemcpyDeviceToHost, st));
+    KS_CUDA(cudaStreamSynchronize(st));
+  }
+  build_table(indptr, n_rows, s->rowt, st);
   build_table(colptr, n_cols, s->colt, st);
   c.check_async("sparse upload (CSC)");
   return s;

@@ -94,6 +94,19 @@ class MulticlassMetrics:
         return self._micro(lambda m: m.fScore(beta))
 
 
+class BinaryClassifierEvaluator:
+    """BinaryClassifierEvaluator (K/evaluation/BinaryClassifierEvaluator.scala): the contingency table of boolean predictions
+    against boolean actuals."""
+
+    @staticmethod
+    def evaluate(predictions, actuals) -> BinaryClassificationMetrics:
+        p = np.asarray(predictions).astype(bool).ravel()
+        a = np.asarray(actuals).astype(bool).ravel()
+        if p.shape != a.shape:
+            raise ValueError("predictions and actuals differ in length")
+        return BinaryClassificationMetrics(float(np.sum(p & a)), float(np.sum(p & ~a)), float(np.sum(~p & ~a)), float(np.sum(~p & a)))
+
+
 class MulticlassClassifierEvaluator:
     """MulticlassClassifierEvaluator(numClasses).  `evaluate_model` runs model -> MaxClassifier -> confusion matrix on the device
     for a fitted BlockLinearMapper and +-1 indicator labels; `from_confusion_matrix` wraps counts obtained elsewhere."""

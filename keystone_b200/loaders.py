@@ -6,14 +6,18 @@ Reference (K/ = src/main/scala/keystoneml/):
   TimitFeaturesDataLoader   K/loaders/TimitFeaturesDataLoader.scala:22-83  feature CSVs + sparse "row label" files (both 1-based)
   CifarLoader               K/loaders/CifarLoader.scala:30-45         records of 1 label byte + 3072 image bytes
   MNIST CSV layout          K/pipelines/images/mnist/MnistRandomFFT.scala:34-36  column 0 = 1-based label, rest = pixels
+  AmazonReviewsDataLoader   K/loaders/AmazonReviewsDataLoader.scala   JSON lines: label = overall >= threshold, data = reviewText
+  NewsgroupsDataLoader      K/loaders/NewsgroupsDataLoader.scala      one directory per class, one document per file
 Parsing happens in the native library (keystone_b200/csrc/io.cu); the arrays returned here are host buffers ready for
 ``Context.matrix`` / ``Context.labels_from_classes``.
 """
 from __future__ import annotations
 
 import ctypes as C
+import json
+import os
 from dataclasses import dataclass
-from typing import Tuple
+from typing import List, Tuple
 
 import numpy as np
 
@@ -76,3 +80,55 @@ def CifarLoader(path: str) -> LabeledData:
     _io_check(lib().ks_cifar_read(path.encode(), images.ctypes.data_as(C.c_void_p), labels.ctypes.data_as(C.c_void_p), n.value,
                                   C.byref(n)))
     return LabeledData(labels=labels, data=images.reshape(n.value, 3, 32, 32))
+
+
+def _json_files(path: str) -> List[str]:
+    if os.path.isdir(path):
+        return [os.path.join(path, f) for f in sorted(os.listdir(path)) if os.path.isfile(os.path.join(path, f)) and not f.startswith((".", "_"))]
+    return [path]
+
+
+def AmazonReviewsDataLoader(path: str, threshold: float) -> LabeledData:
+    """The Amazon product reviews (AmazonReviewsDataLoader.scala): JSON records, one per line, from one file or from every file of a
+    directory in sorted name order.  ``labels[i]`` is 1 when record i's ``overall`` is >= ``threshold``, else 0; ``data`` is the list
+    of its ``reviewText`` strings.  A record without either field raises ``ValueError`` naming the file and line."""
+    labels: List[int] = []
+    docs: List[str] = []
+    for f in _json_files(path):
+        with open(f, encoding="utf-8") as fh:
+            for ln, line in enumerate(fh, 1):
+                if not line.strip():
+                    continue
+                rec = json.loads(line)
+                if not isinstance(rec, dict) or "overall" not in rec or "reviewText" not in rec:
+                    raise ValueError(f"{f}:{ln}: a review needs the fields overall and reviewText")
+                labels.append(1 if float(rec["overall"]) >= threshold else 0)
+                docs.append(str(rec["reviewText"]))
+    return LabeledData(np.asarray(labels, dtype=np.int32), docs)
+
+
+class NewsgroupsDataLoader:
+    """The 20 Newsgroups documents (NewsgroupsDataLoader.scala): ``NewsgroupsDataLoader(path)`` returns ``LabeledData`` whose data
+    holds every file of ``path/<class>/`` for the classes below in order, files in sorted name order, decoded as UTF-8 with invalid
+    bytes replaced by U+FFFD (as Hadoop's ``Text`` decodes them); the label is the class index.  A missing class directory raises
+    ``FileNotFoundError``, as the reference's ``wholeTextFiles`` fails on a missing path."""
+
+    classes = ["comp.graphics", "comp.os.ms-windows.misc", "comp.sys.ibm.pc.hardware", "comp.sys.mac.hardware", "comp.windows.x",
+               "rec.autos", "rec.motorcycles", "rec.sport.baseball", "rec.sport.hockey", "sci.crypt", "sci.electronics", "sci.med",
+               "sci.space", "misc.forsale", "talk.politics.misc", "talk.politics.guns", "talk.politics.mideast", "talk.religion.misc",
+               "alt.atheism", "soc.religion.christian"]
+
+    def __new__(cls, path: str) -> LabeledData:
+        labels: List[int] = []
+        docs: List[str] = []
+        for k, name in enumerate(cls.classes):
+            d = os.path.join(path, name)
+            if not os.path.isdir(d):
+                raise FileNotFoundError(f"{d}: the class directory {name!r} is missing")
+            for f in sorted(os.listdir(d)):
+                fp = os.path.join(d, f)
+                if os.path.isfile(fp):
+                    with open(fp, "rb") as fh:
+                        docs.append(fh.read().decode("utf-8", "replace"))
+                    labels.append(k)
+        return LabeledData(np.asarray(labels, dtype=np.int32), docs)

@@ -23,6 +23,11 @@ Reference classes (K/ = src/main/scala/keystoneml/):
   Densify                             K/nodes/util/Densify.scala
   LogisticRegressionEstimator / Model K/nodes/learning/LogisticRegressionModel.scala
   NaiveBayesEstimator / Model         K/nodes/learning/NaiveBayesModel.scala
+  Trim, LowerCase, Tokenizer          K/nodes/nlp/StringUtils.scala (text front end, DESIGN.md section 23)
+  NGramsFeaturizer                    K/nodes/nlp/ngrams.scala
+  TermFrequency                       K/nodes/stats/TermFrequency.scala
+  CommonSparseFeatures, AllSparseFeatures, SparseFeatureVectorizer   K/nodes/util/*.scala
+  HashingTF, NGramsHashingTF          K/nodes/nlp/{HashingTF,NGramsHashingTF}.scala
 
 Batches are ``DeviceMatrix`` / ``LazyFeatures`` (this rank's rows); 2-D numpy arrays are uploaded on
 the fly when a ``Context`` was given to the node.  No node computes on the host.
@@ -37,7 +42,8 @@ import numpy as np
 
 from . import _capi
 from ._capi import KeystoneError, check, lib
-from .context import Context, Dataset, DeviceMatrix, LazyFeatures, SparseMatrix, feature_source_args
+from .context import (Context, Dataset, DeviceMatrix, LazyFeatures, NGramBatch, SparseMatrix, TermFrequencyBatch, TextBatch, TokenBatch,
+                      _flatten_terms, _host_terms, feature_source_args)
 from .workflow import Estimator, LabelEstimator, Transformer, WeightedNode
 
 
@@ -2400,3 +2406,272 @@ def _gather_rows(x: DeviceMatrix, rows: np.ndarray) -> DeviceMatrix:
     h = C.c_int64(0)
     check(x.ctx.handle, lib().ks_matrix_gather_rows(x.ctx.handle, x.handle, rows.ctypes.data_as(C.c_void_p), rows.size, C.byref(h)))
     return DeviceMatrix(x.ctx, h.value, rows.size, x.cols)
+
+
+# ------------------------------------------------------------------------------------------ the text front end (DESIGN.md section 23)
+def _as_text(ctx: Optional[Context], data) -> TextBatch:
+    if isinstance(data, TextBatch):
+        return data
+    if isinstance(data, Dataset):
+        raise KeystoneError(-1, f"a text node needs a TextBatch, not {type(data).__name__}")
+    if ctx is None:
+        raise KeystoneError(-1, "host documents need a Context (pass ctx= to the node)")
+    return ctx.text(list(data))
+
+
+def _as_terms(ctx: Optional[Context], data):
+    """(token batch, min order, max order) of a batch of terms: a ``TokenBatch`` (its tokens as terms, orders 0, 0), an ``NGramBatch``,
+    or host lists of ``str`` tokens.  Host lists of n-gram tuples are rejected: n-grams reach the device as an ``NGramBatch``."""
+    if isinstance(data, NGramBatch):
+        return data.tokens, data.min_order, data.max_order
+    if isinstance(data, TokenBatch):
+        return data, 0, 0
+    if isinstance(data, Dataset):
+        raise KeystoneError(-1, f"a term node needs a TokenBatch or an NGramBatch, not {type(data).__name__}")
+    if ctx is None:
+        raise KeystoneError(-1, "host token lists need a Context (pass ctx= to the node)")
+    docs = [list(d) for d in data]
+    if any(isinstance(t, tuple) for d in docs for t in d):
+        # the device emits n-grams from tokens; arbitrary host tuples have no token batch and orders to be emitted from
+        raise KeystoneError(-1, "host lists of n-gram tuples are not accepted: pass the tokens through NGramsFeaturizer, which gives "
+                                "an NGramBatch")
+    return ctx.tokens(docs), 0, 0
+
+
+def _as_tf(ctx: Optional[Context], data) -> TermFrequencyBatch:
+    if isinstance(data, TermFrequencyBatch):
+        return data
+    if isinstance(data, Dataset):
+        raise KeystoneError(-1, f"this node needs a TermFrequencyBatch, not {type(data).__name__}")
+    if ctx is None:
+        raise KeystoneError(-1, "host term-frequency lists need a Context (pass ctx= to the node)")
+    return ctx.term_frequencies([list(d) for d in data])
+
+
+def _check_orders(orders) -> tuple:
+    """NGramsFeaturizer's requirements (ngrams.scala): orders >= 1 and consecutive, in increasing order."""
+    o = [int(x) for x in orders]
+    if not o:
+        raise ValueError("orders must not be empty")
+    if min(o) < 1:
+        raise ValueError(f"minimum order is not >= 1, found {min(o)}")
+    for a, b in zip(o, o[1:]):
+        if a != b - 1:
+            raise ValueError(f"orders are not consecutive; contains {a} and {b}")
+    return o[0], o[-1]
+
+
+def _sparse_result(ctx: Context, handle: int) -> SparseMatrix:
+    rows, cols, nnz = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+    check(ctx.handle, lib().ks_sparse_shape(ctx.handle, handle, C.byref(rows), C.byref(cols), C.byref(nnz)))
+    return SparseMatrix(ctx, handle, rows.value, cols.value, nnz.value)
+
+
+def _transform_text(ctx: Optional[Context], data, flags: int) -> TextBatch:
+    t = _as_text(ctx, data)
+    h = C.c_int64(0)
+    check(t.ctx.handle, lib().ks_text_transform(t.ctx.handle, t.handle, flags, C.byref(h)))
+    return TextBatch(t.ctx, h.value, t.n_docs)
+
+
+class Trim(Transformer):
+    """``Trim`` (K/nodes/nlp/StringUtils.scala): Java's ``String.trim``, which strips leading and trailing code points <= U+0020."""
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx
+
+    def apply(self, data) -> TextBatch:
+        return _transform_text(self.ctx, data, _capi.KS_TEXT_TRIM)
+
+
+class LowerCase(Transformer):
+    """``LowerCase(locale)`` (K/nodes/nlp/StringUtils.scala) in the root locale: every code point by its one-to-one Unicode lowercase
+    mapping, and U+0130 to "i" U+0307 as Java does.  Java's final-sigma rule is not applied (a final capital sigma becomes U+03C3).
+    The Turkish, Azeri and Lithuanian locales, whose rules differ, are rejected."""
+
+    def __init__(self, locale: Optional[str] = None, ctx: Optional[Context] = None):
+        if locale is not None and str(locale).replace("-", "_").split("_")[0].lower() in ("tr", "az", "lt"):
+            raise ValueError(f"LowerCase: the {locale} locale has its own lowercase rules, which are not implemented")
+        self.locale, self.ctx = locale, ctx
+
+    def apply(self, data) -> TextBatch:
+        return _transform_text(self.ctx, data, _capi.KS_TEXT_LOWER)
+
+
+class Tokenizer(Transformer):
+    """``Tokenizer(sep)`` (K/nodes/nlp/StringUtils.scala) with the default pattern ``[\\p{Punct}\\s]+`` only: Java's
+    ``String.split`` on runs of ASCII punctuation and whitespace.  A leading separator gives a leading "", trailing empty strings
+    are dropped, "" gives [""] and a document of separators only gives []."""
+
+    DEFAULT_SEP = "[\\p{Punct}\\s]+"
+
+    def __init__(self, sep: str = DEFAULT_SEP, ctx: Optional[Context] = None):
+        if sep != self.DEFAULT_SEP:
+            raise ValueError(f"Tokenizer: only the default separator {self.DEFAULT_SEP!r} is implemented, not {sep!r}")
+        self.sep, self.ctx = sep, ctx
+
+    def apply(self, data) -> TokenBatch:
+        t = _as_text(self.ctx, data)
+        h = C.c_int64(0)
+        check(t.ctx.handle, lib().ks_text_tokenize(t.ctx.handle, t.handle, C.byref(h)))
+        return TokenBatch(t.ctx, h.value, t.n_docs)
+
+
+class NGramsFeaturizer(Transformer):
+    """``NGramsFeaturizer(orders)`` (K/nodes/nlp/ngrams.scala): the n-grams of every document as tuples, for each position i and
+    then each order.  The result is an ``NGramBatch``, emitted on the device by the node that consumes it; ``TermFrequency`` takes
+    orders up to 4, the hashing nodes any order."""
+
+    def __init__(self, orders, ctx: Optional[Context] = None):
+        self.min_order, self.max_order = _check_orders(orders)
+        self.orders, self.ctx = list(range(self.min_order, self.max_order + 1)), ctx
+
+    def apply(self, data) -> NGramBatch:
+        tokens, mn, _ = _as_terms(self.ctx, data)
+        if mn != 0:
+            raise KeystoneError(-1, "NGramsFeaturizer takes tokens, not n-grams")
+        return NGramBatch(tokens, self.min_order, self.max_order)
+
+
+def _identity(x):
+    return x
+
+
+class TermFrequency(Transformer):
+    """``TermFrequency(fun)`` (K/nodes/stats/TermFrequency.scala): per document its distinct terms, in order of first occurrence,
+    each with ``fun(count)``.  The device counts; ``fun`` is evaluated on the host once for every count 1 .. the largest count in the
+    batch, and a result that is not finite is rejected.  Input: a ``TokenBatch``, an ``NGramBatch`` or host lists of ``str`` tokens
+    (host lists of n-gram tuples are rejected; use ``NGramsFeaturizer`` on the tokens)."""
+
+    def __init__(self, fun=_identity, ctx: Optional[Context] = None):
+        self.fun, self.ctx = fun, ctx
+
+    def apply(self, data) -> TermFrequencyBatch:
+        tokens, mn, mx = _as_terms(self.ctx, data)
+        ctx = tokens.ctx
+        h, mc = C.c_int64(0), C.c_int64(0)
+        check(ctx.handle, lib().ks_term_frequency(ctx.handle, tokens.handle, mn, mx, C.byref(h), C.byref(mc)))
+        tf = TermFrequencyBatch(ctx, h.value, tokens.n_docs, tokens, mc.value)
+        if self.fun is not _identity and mc.value > 0:
+            table = np.array([float(self.fun(float(c))) for c in range(1, mc.value + 1)], dtype=np.float64)
+            bad = np.flatnonzero(~np.isfinite(table))
+            if bad.size:
+                raise KeystoneError(-1, f"TermFrequency: fun({int(bad[0]) + 1}) = {table[bad[0]]} is not finite")
+            check(ctx.handle, lib().ks_tf_set_weights(ctx.handle, tf.handle, table.ctypes.data_as(C.c_void_p), table.shape[0]))
+        return tf
+
+
+class SparseFeatureVectorizer(Transformer):
+    """``SparseFeatureVectorizer(featureSpace)`` (K/nodes/util/SparseFeatureVectorizer.scala): ``apply`` maps every document's
+    ``(term, value)`` pairs to a ``SparseMatrix`` row with ``len(feature_space)`` columns, fp64 values, columns ascending; terms
+    outside the space are dropped, and a term repeated within one document of a host list gives one entry, the sum of its values.  Terms match by their bytes.  ``SparseFeatureVectorizer(feature_space, ctx=ctx)`` uploads a host
+    ``{term: column}`` dict whose columns are 0 .. n-1; ``feature_space`` reads the fitted space back as such a dict."""
+
+    def __init__(self, feature_space, ctx: Optional[Context] = None, _handle: int = 0):
+        if _handle:
+            self.ctx, self.handle = ctx, _handle
+            n = C.c_int64(0)
+            check(ctx.handle, lib().ks_text_array_size(ctx.handle, _handle, _capi.KS_TEXT_TERM_ORDER, C.byref(n)))
+            self.num_features = n.value
+            return
+        if ctx is None:
+            raise KeystoneError(-1, "SparseFeatureVectorizer from a host feature space needs a Context (pass ctx=)")
+        items = sorted(dict(feature_space).items(), key=lambda kv: kv[1])
+        if [v for _, v in items] != list(range(len(items))):
+            raise ValueError("the feature space's columns must be 0 .. len(feature_space) - 1")
+        tokens, first, order = _flatten_terms([k for k, _ in items])
+        tk = ctx.tokens([tokens])
+        h = C.c_int64(0)
+        check(ctx.handle, lib().ks_sparse_features_from_host(ctx.handle, tk.handle, first.ctypes.data_as(C.c_void_p),
+                                                              order.ctypes.data_as(C.c_void_p), len(items), C.byref(h)))
+        self.ctx, self.handle, self.num_features = ctx, h.value, len(items)
+
+    @property
+    def feature_space(self) -> dict:
+        return {t: i for i, t in enumerate(_host_terms(self.ctx, self.handle))}
+
+    def apply(self, data) -> SparseMatrix:
+        tf = _as_tf(self.ctx, data)
+        h = C.c_int64(0)
+        check(self.ctx.handle, lib().ks_sparse_features_apply(self.ctx.handle, self.handle, tf.handle, C.byref(h)))
+        return _sparse_result(self.ctx, h.value)
+
+    def __del__(self):
+        try:
+            if self.handle and self.ctx.handle:
+                lib().ks_text_destroy(self.ctx.handle, self.handle)
+        except Exception:
+            pass
+
+
+def _fit_space(ctx: Optional[Context], data, num_features: int) -> SparseFeatureVectorizer:
+    tf = _as_tf(ctx, data)
+    if tf.ctx.world_size > 1:
+        raise KeystoneError(-1, "CommonSparseFeatures / AllSparseFeatures fit on one rank only: an exact top-K over ranks is not implemented")
+    h = C.c_int64(0)
+    check(tf.ctx.handle, lib().ks_sparse_features_fit(tf.ctx.handle, tf.handle, num_features, C.byref(h)))
+    return SparseFeatureVectorizer(None, tf.ctx, _handle=h.value)
+
+
+class CommonSparseFeatures(Estimator):
+    """``CommonSparseFeatures(numFeatures)`` (K/nodes/util/CommonSparseFeatures.scala): ``fit`` keeps the ``num_features`` terms
+    held by the most entries (document frequency), ties by earliest appearance in the flattened batch, and returns a
+    ``SparseFeatureVectorizer``.  One rank only."""
+
+    def __init__(self, num_features: int, ctx: Optional[Context] = None):
+        if int(num_features) < 1:
+            raise ValueError("num_features must be >= 1")
+        self.num_features, self.ctx = int(num_features), ctx
+
+    def fit(self, data) -> SparseFeatureVectorizer:
+        return _fit_space(self.ctx, data, self.num_features)
+
+
+class AllSparseFeatures(Estimator):
+    """``AllSparseFeatures()`` (K/nodes/util/AllSparseFeatures.scala): every term, in the order of ``CommonSparseFeatures`` without a
+    cut.  One rank only."""
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx
+
+    def fit(self, data) -> SparseFeatureVectorizer:
+        return _fit_space(self.ctx, data, -1)
+
+
+def _hashing_tf(ctx: Optional[Context], data, num_features: int, orders=None) -> SparseMatrix:
+    tokens, mn, mx = _as_terms(ctx, data)
+    if orders is not None:
+        if mn != 0:
+            raise KeystoneError(-1, "NGramsHashingTF takes tokens, not n-grams")
+        mn, mx = orders
+    h = C.c_int64(0)
+    check(tokens.ctx.handle, lib().ks_hashing_tf(tokens.ctx.handle, tokens.handle, mn, mx, num_features, C.byref(h)))
+    return _sparse_result(tokens.ctx, h.value)
+
+
+class HashingTF(Transformer):
+    """``HashingTF(numFeatures)`` (K/nodes/nlp/HashingTF.scala): term counts at column ``nonNegativeMod(term.##, numFeatures)``:
+    ``String.hashCode`` for the tokens of a ``TokenBatch`` (or host lists of ``str``), ``MurmurHash3.seqHash`` for the tuples of an
+    ``NGramBatch``.  Host lists of n-gram tuples are rejected; use ``NGramsFeaturizer`` on the tokens."""
+
+    def __init__(self, num_features: int, ctx: Optional[Context] = None):
+        if not 1 <= int(num_features) < 2 ** 31:
+            raise ValueError("num_features must lie in [1, 2^31 - 1]")
+        self.num_features, self.ctx = int(num_features), ctx
+
+    def apply(self, data) -> SparseMatrix:
+        return _hashing_tf(self.ctx, data, self.num_features)
+
+
+class NGramsHashingTF(Transformer):
+    """``NGramsHashingTF(orders, numFeatures)`` (K/nodes/nlp/NGramsHashingTF.scala): the same counts as ``NGramsFeaturizer(orders)
+    andThen HashingTF(numFeatures)`` without forming the n-grams; any order."""
+
+    def __init__(self, orders, num_features: int, ctx: Optional[Context] = None):
+        self.min_order, self.max_order = _check_orders(orders)
+        if not 1 <= int(num_features) < 2 ** 31:
+            raise ValueError("num_features must lie in [1, 2^31 - 1]")
+        self.num_features, self.ctx = int(num_features), ctx
+
+    def apply(self, data) -> SparseMatrix:
+        return _hashing_tf(self.ctx, data, self.num_features, (self.min_order, self.max_order))

@@ -1,5 +1,6 @@
 """The CIFAR random-patch pipelines of the reference on the device (K/pipelines/images/cifar/RandomPatchCifar.scala,
-RandomPatchCifarAugmented.scala).  DESIGN.md section 21.
+RandomPatchCifarAugmented.scala), DESIGN.md section 21, and the text pipelines (K/pipelines/text/AmazonReviewsPipeline.scala,
+NewsgroupsPipeline.scala), DESIGN.md section 23.
 
 Filter learning: ``Windower -> ImageVectorizer -> Sampler(whitenerSize) -> Stats.normalizeRows(., 10) -> ZCAWhitenerEstimator ->
 sampleRows(numFilters) -> whiten -> unit norm -> . whitener^T``.  Everything with a row per window, view or image runs on the device;
@@ -14,7 +15,9 @@ from typing import Optional
 import numpy as np
 
 from .context import Context, DeviceMatrix
-from .evaluation import AugmentedExamplesEvaluator, MulticlassClassifierEvaluator
+from .evaluation import AugmentedExamplesEvaluator, BinaryClassifierEvaluator, MulticlassClassifierEvaluator
+from .nodes import (CommonSparseFeatures, LogisticRegressionEstimator, LowerCase, MaxClassifier, NaiveBayesEstimator, NGramsFeaturizer,
+                    TermFrequency, Tokenizer, Trim)
 from .nodes import (BlockLeastSquaresEstimator, BlockLinearMapper, CenterCornerPatcher, Convolver, ImageBatch, ImageVectorizer, Pooler,
                     RandomImageTransformer, RandomPatcher, Sampler, StandardScaler, StandardScalerModel, SymmetricRectifier, Windower,
                     ZCAWhitenerEstimator, cifar_bytes_to_matrix, flip_horizontal, sample_rows, stats_normalize_rows)
@@ -96,7 +99,7 @@ def _fit(ctx: Context, train_images, train_classes: np.ndarray, filters, W, mean
 
 def _single_rank(ctx: Context) -> None:
     if ctx.world_size > 1:
-        raise NotImplementedError("the CIFAR pipelines run on one rank")
+        raise NotImplementedError("the CIFAR and text pipelines run on one rank")
 
 
 def random_patch_cifar(ctx: Context, train, test, conf: Optional[RandomCifarFeaturizerConfig] = None):
@@ -133,3 +136,60 @@ def random_patch_cifar_augmented(ctx: Context, train, test, conf: Optional[Rando
     scores = fitted.apply(test_views)
     test_eval = AugmentedExamplesEvaluator(names, NUM_CLASSES).evaluate(scores, np.repeat(np.asarray(test.labels), NUM_TEST_AUGMENT))
     return fitted, train_eval, test_eval
+
+
+# ------------------------------------------------------------------------------------------ text pipelines (DESIGN.md section 23)
+@dataclass
+class AmazonReviewsConfig:
+    """``AmazonReviewsConfig``'s defaults without the file locations and ``numParts``."""
+    threshold: float = 3.5
+    nGrams: int = 2
+    commonFeatures: int = 100000
+    numIters: int = 20
+
+
+@dataclass
+class NewsgroupsConfig:
+    nGrams: int = 2
+    commonFeatures: int = 100000
+
+
+def _one(x):
+    return 1.0
+
+
+def _text_featurizer(ctx: Context, train_docs, n_grams: int, common_features: int):
+    """``Trim andThen LowerCase() andThen Tokenizer() andThen NGramsFeaturizer(1 to n) andThen TermFrequency(x => 1) andThen
+    (CommonSparseFeatures(k), train)``"""
+    return (Trim(ctx=ctx).andThen(LowerCase()).andThen(Tokenizer()).andThen(NGramsFeaturizer(range(1, n_grams + 1)))
+            .andThen(TermFrequency(_one)).andThen(CommonSparseFeatures(common_features), train_docs))
+
+
+def amazon_reviews_pipeline(ctx: Context, train, test, conf: Optional[AmazonReviewsConfig] = None):
+    """``AmazonReviewsPipeline.run``: train and test are ``LabeledData`` as ``AmazonReviewsDataLoader`` returns them.  Logistic
+    regression (2 classes, ``numIters``) on the common n-gram features; returns (fitted predictor, test
+    ``BinaryClassificationMetrics`` of prediction > 0 against label > 0)."""
+    _single_rank(ctx)
+    conf = conf or AmazonReviewsConfig()
+    train_docs = ctx.text(list(train.data))
+    labels = np.asarray(train.labels)
+    predictor = _text_featurizer(ctx, train_docs, conf.nGrams, conf.commonFeatures).andThen(
+        LogisticRegressionEstimator(num_classes=2, num_iters=conf.numIters), train_docs, labels).fit()
+    results = predictor(ctx.text(list(test.data)))
+    return predictor, BinaryClassifierEvaluator.evaluate(np.asarray(results) > 0, np.asarray(test.labels) > 0)
+
+
+def newsgroups_pipeline(ctx: Context, train, test, conf: Optional[NewsgroupsConfig] = None):
+    """``NewsgroupsPipeline.run``: train and test are ``LabeledData`` as ``NewsgroupsDataLoader`` returns them.  Naive Bayes over the
+    20 classes, then ``MaxClassifier``; returns (fitted predictor, test ``MulticlassMetrics``)."""
+    from .loaders import NewsgroupsDataLoader
+    _single_rank(ctx)
+    conf = conf or NewsgroupsConfig()
+    k = len(NewsgroupsDataLoader.classes)
+    train_docs = ctx.text(list(train.data))
+    predictor = _text_featurizer(ctx, train_docs, conf.nGrams, conf.commonFeatures).andThen(
+        NaiveBayesEstimator(k), train_docs, np.asarray(train.labels)).andThen(MaxClassifier()).fit()
+    pred = np.asarray(predictor(ctx.text(list(test.data))))
+    cm = np.zeros((k, k), dtype=np.float64)
+    np.add.at(cm, (np.asarray(test.labels, dtype=np.int64), pred.astype(np.int64)), 1.0)
+    return predictor, MulticlassClassifierEvaluator.from_confusion_matrix(cm)

@@ -46,6 +46,27 @@ class KeystoneB200 extends Serializable {
   @native def logisticFit(ctx: Long, features: Long, sparse: Long, classes: Array[Int], numClasses: Int, regParam: Double, numIters: Int,
       convergenceTol: Double): Long
   @native def naiveBayesFit(ctx: Long, features: Long, sparse: Long, classes: Array[Int], numClasses: Int, lambda: Double): Long
+  /** The text front end (DESIGN.md section 23; not collective): UTF-8 bytes with Long offsets in, text-object handles out (released
+   *  by textDestroy).  termFrequency returns (handle, largest count); textArray* read a KS_TEXT_* array of an object back;
+   *  sparseFeaturesApply and hashingTf return sparse matrix handles, read by sparseToHostCsr as (indptr, indices, values). */
+  @native def textFromHost(ctx: Long, bytes: Array[Byte], docOffsets: Array[Long]): Long
+  @native def textTransform(ctx: Long, text: Long, flags: Int): Long
+  @native def textTokenize(ctx: Long, text: Long): Long
+  @native def tokensFromHost(ctx: Long, bytes: Array[Byte], tokenOffsets: Array[Long], docOffsets: Array[Long]): Long
+  @native def termFrequency(ctx: Long, tokens: Long, minOrder: Int, maxOrder: Int): Array[Long]
+  @native def tfSetWeights(ctx: Long, tf: Long, table: Array[Double]): Unit
+  @native def tfFromHost(ctx: Long, tokens: Long, termFirst: Array[Long], termOrder: Array[Int], values: Array[Double],
+      docOffsets: Array[Long]): Long
+  @native def sparseFeaturesFit(ctx: Long, tf: Long, numFeatures: Long): Long
+  @native def sparseFeaturesFromHost(ctx: Long, tokens: Long, termFirst: Array[Long], termOrder: Array[Int]): Long
+  @native def sparseFeaturesApply(ctx: Long, space: Long, tf: Long): Long
+  @native def hashingTf(ctx: Long, tokens: Long, minOrder: Int, maxOrder: Int, numFeatures: Long): Long
+  @native def textArrayBytes(ctx: Long, obj: Long, which: Int): Array[Byte]
+  @native def textArrayInts(ctx: Long, obj: Long, which: Int): Array[Int]
+  @native def textArrayLongs(ctx: Long, obj: Long, which: Int): Array[Long]
+  @native def textArrayDoubles(ctx: Long, obj: Long, which: Int): Array[Double]
+  @native def textDestroy(ctx: Long, obj: Long): Unit
+  @native def sparseToHostCsr(ctx: Long, s: Long): Array[AnyRef]
   /** PCA / ZCA / approximate PCA (collective, fp64 on the device); omega is the d x l test matrix, DenseMatrix.data. */
   @native def pcaFit(ctx: Long, x: Long, dims: Int): Long
   @native def zcaFit(ctx: Long, x: Long, eps: Double): Long
